@@ -1,5 +1,5 @@
 /*
- * mkb200.h -- C-ABI of libmkb200.so: the B200-native voxel-occupancy and trajectory-distance engine.
+ * mkb200.h -- C-ABI of libmkb200.so: the H100-native voxel-occupancy and trajectory-distance engine.
  *
  * This is the drop-in boundary for ONE hot path of Acellera/moleculekit (SURVEY.md section 8):
  *   moleculekit/occupancy_utils/occupancy_utils.pyx   (calculate_occupancy)

@@ -1,4 +1,4 @@
-"""moleculekit_b200 -- B200-native voxel-descriptor and trajectory-distance engine.
+"""moleculekit_b200 -- H100-native voxel-descriptor and trajectory-distance engine.
 
 Drop-in for ONE hot path of Acellera/moleculekit (SURVEY.md section 8):
 
@@ -6,7 +6,7 @@ Drop-in for ONE hot path of Acellera/moleculekit (SURVEY.md section 8):
     moleculekit.projections.metricdistance.MetricDistance / MetricSelfDistance (.project)
     moleculekit.occupancy_utils / moleculekit.distance_utils (the Cython kernels underneath)
 
-Python host code -> ctypes C-ABI (include/mkb200.h) -> hand-written CUDA kernels for sm_100a.
+Python host code -> ctypes C-ABI (include/mkb200.h) -> hand-written CUDA kernels for sm_90a (H100).
 PyTorch tensors are the device container only.  There is no CPU fallback.
 """
 __version__ = "0.1.0"

@@ -1,4 +1,4 @@
-// bonds.cu -- K7 (SURVEY row a13, stretch): bond perception on a uniform non-periodic cell grid for sm_100a.
+// bonds.cu -- K7 (SURVEY row a13, stretch): bond perception on a uniform non-periodic cell grid for sm_90a (H100).
 //
 // Replaces moleculekit/bondguesser.py:259-392 (bond_grid_search: Python dict binning + one Cython call per occupied
 // box) and moleculekit/bondguesser_utils/bondguesser_utils.pyx:30-163 (half-shell neighbour table, _is_close,

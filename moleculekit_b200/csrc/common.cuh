@@ -49,7 +49,7 @@ struct mkb_ctx {
     mkb::Scratch scratch[mkb::S_NSLOTS];
     int64_t launches = 0;
     const char *last_kernel = "";  // main kernel of the most recent occupancy / distance call (bench.py's roofline.kernel)
-    int sm_count = 148;
+    int sm_count = 132;
     // optional per-kernel timing (bench.py roofline): events recorded on the launch stream
     bool timing = false;
     cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};  // before prep, before main kernel, after main kernel

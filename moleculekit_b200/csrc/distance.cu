@@ -1,4 +1,4 @@
-// distance.cu -- K3/K4/K5/K6: trajectory distances, ordered contacts, group reductions, cdist/pdist for sm_100a.
+// distance.cu -- K3/K4/K5/K6: trajectory distances, ordered contacts, group reductions, cdist/pdist for sm_90a (H100).
 //
 // Replaces moleculekit/distance_utils/distance_utils.pyx (all functions) with the post-ops of
 // moleculekit/projections/util.py:74-84,212-223 fused into the stores.
@@ -40,33 +40,6 @@ __device__ __forceinline__ float wrap_axis(float d, float b, float rb) {
 
 __device__ __forceinline__ float sq3(float dx, float dy, float dz) {
     return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-}
-
-// packed float32 pairs (sm_100): a 64-bit register holds (lo, hi); used by the contact-map estimate of K3
-#ifndef MKB_K3_X2
-#define MKB_K3_X2 1  // measured on C4a contacts: 3.705 -> 3.538 ms, same booleans (23 distance GPU tests)
-#endif
-typedef unsigned long long f2_t;
-__device__ __forceinline__ f2_t f2_pack(float lo, float hi) {
-    f2_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void f2_unpack(f2_t v, float &lo, float &hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f2_t f2_fma(f2_t a, f2_t b, f2_t c) {
-    f2_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-__device__ __forceinline__ f2_t f2_mul(f2_t a, f2_t b) {
-    f2_t r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ f2_t f2_add(f2_t a, f2_t b) {
-    f2_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
 }
 
 struct BoxF {
@@ -297,8 +270,6 @@ __device__ __forceinline__ void emit_dist(void *out, long long idx, float d2, fl
 // Each thread owns TWO sel2 columns (j and j + K3_COLS) so one broadcast load of the sel1 atom, the loop control and the
 // index arithmetic are shared by two pairs.  SELF / PBC are compile-time: the rectangular non-periodic-free inner loop
 // carries no per-row diagonal tests.
-// (register sweep, C4a: compiler default 4.85 / 4.32 ms distances / contacts; forced 32 regs 5.10 / 4.89; 40 regs with the
-// box halves pinned 4.79 / 4.62; 48 regs 4.81 / 4.62; 61 regs 5.07 / 4.27 -- within noise of the default, which stays)
 #ifdef MKB_K3_MIN_CTAS
 #define MKB_K3_BOUNDS __launch_bounds__(K3_COLS, MKB_K3_MIN_CTAS)
 #else
@@ -327,50 +298,6 @@ __global__ void MKB_K3_BOUNDS dist_kernel(const float4 *__restrict__ G1, const f
         unsigned char *const o8 = reinterpret_cast<unsigned char *>(out);
         long long idx = f * P + (SELF ? (i0 * n2 - (i0 * (i0 + 1)) / 2 + (j0 - i0 - 1)) : (i0 * n2 + j0));
         long long step = SELF ? n2 - i0 - 2 : n2;
-#if MKB_K3_X2
-        // The thread's two pairs of a row as PACKED float32 pairs (sm_100 add / mul / fma .f32x2): the estimate of pair_contact,
-        // operation for operation, on (pair 0, pair 1) -- half the FMA-pipe issue slots.  Only the ESTIMATE is packed: ptxas
-        // contracts packed mul + add into FFMA2 (even with .rn and -fmad=false), which an estimate tolerates (any nearest
-        // integer of a quotient good to 1e-6 satisfies the argument above) and the exact sequence would not.
-        if (!SELF && has1 && shortcut) {
-            const f2_t nbx = f2_pack(-b0.x, -b1.x), nby = f2_pack(-b0.y, -b1.y), nbz = f2_pack(-b0.z, -b1.z);
-            const f2_t M2 = f2_pack(12582912.0f, 12582912.0f), NM2 = f2_pack(-12582912.0f, -12582912.0f);
-            const float band = 4e-6f * threshold;
-            for (int r = 0; r < rows; ++r) {
-                const float4 a = __ldg(arow + r);
-                const unsigned ca = __float_as_uint(a.w);
-                const bool w0 = pbc && ca != cb0, w1 = pbc && ca != cb1;
-                bool c0, c1;
-                if (w0 == w1) {
-                    f2_t dx = f2_add(f2_pack(a.x, a.x), nbx), dy = f2_add(f2_pack(a.y, a.y), nby), dz = f2_add(f2_pack(a.z, a.z), nbz);
-                    float qm0 = 0.0f, qm1 = 0.0f;
-                    if (w0) {
-                        const f2_t qx = f2_mul(dx, f2_pack(bx.rx, bx.rx)), qy = f2_mul(dy, f2_pack(bx.ry, bx.ry)),
-                                   qz = f2_mul(dz, f2_pack(bx.rz, bx.rz));
-                        dx = f2_fma(f2_pack(-bx.bx, -bx.bx), f2_add(f2_add(qx, M2), NM2), dx);
-                        dy = f2_fma(f2_pack(-bx.by, -bx.by), f2_add(f2_add(qy, M2), NM2), dy);
-                        dz = f2_fma(f2_pack(-bx.bz, -bx.bz), f2_add(f2_add(qz, M2), NM2), dz);
-                        float x0, x1, y0, y1, z0, z1;
-                        f2_unpack(qx, x0, x1); f2_unpack(qy, y0, y1); f2_unpack(qz, z0, z1);
-                        qm0 = fmaxf(fmaxf(fabsf(x0), fabsf(y0)), fabsf(z0));
-                        qm1 = fmaxf(fmaxf(fabsf(x1), fabsf(y1)), fabsf(z1));
-                    }
-                    float e0, e1;
-                    f2_unpack(f2_fma(dx, dx, f2_fma(dy, dy, f2_mul(dz, dz))), e0, e1);
-                    // decided unless the estimate is within the band, not a number, or the magic rounding left its range
-                    c0 = (fabsf(e0 - threshold) > band && qm0 < 2097152.0f) ? (e0 <= threshold) : (pair_d2_fastwrap(a, b0, cb0, bx, pbc) <= threshold);
-                    c1 = (fabsf(e1 - threshold) > band && qm1 < 2097152.0f) ? (e1 <= threshold) : (pair_d2_fastwrap(a, b1, cb1, bx, pbc) <= threshold);
-                } else {
-                    c0 = pair_contact(a, b0, cb0, bx, pbc, threshold, shortcut);
-                    c1 = pair_contact(a, b1, cb1, bx, pbc, threshold, shortcut);
-                }
-                o8[idx] = c0 ? 1 : 0;
-                o8[idx + K3_COLS] = c1 ? 1 : 0;
-                idx += step;
-            }
-            return;
-        }
-#endif
 #pragma unroll 2
         for (int r = 0; r < rows; ++r) {
             const float4 a = __ldg(arow + r);

@@ -1,4 +1,4 @@
-// hbonds.cu -- K12: hydrogen-bond detection over a trajectory for sm_100a.
+// hbonds.cu -- K12: hydrogen-bond detection over a trajectory for sm_90a (H100).
 //
 // Replaces hbonds.calculate (moleculekit/interactions/hbonds/hbonds.pyx:25-134), the kernel under hbonds_calculate
 // (moleculekit/interactions/interactions.py:365-467).  Per frame the reference walks donors x acceptors (donor major) and

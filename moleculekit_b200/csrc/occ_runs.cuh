@@ -1,7 +1,6 @@
 // occ_runs.cuh -- K1, the default 8-channel occupancy fill (v10): per-block candidate lists + a persistent "mask-run" kernel.
 // Included by occupancy.cu (after GridDev / occ_value).  Replaces the inner loop of
-// moleculekit/occupancy_utils/occupancy_utils.pyx:46-61.  DESIGN.md section 3 has the derivations, section 5 the
-// measurements of every step (v6 -> v10: 1.82 -> 0.66 ms per 256 pockets of BASELINE config 3); the superseded variants
+// moleculekit/occupancy_utils/occupancy_utils.pyx:46-61.  DESIGN.md section 3 has the derivations; the superseded variants
 // (float-compare gate with predicated FMNMX, scalar FFMA hot loop, row-copy stores, in-register record gathers, jump-table
 // flush, FFMA.SAT gate ...) are in the git history of this file together with their compile-time selectors.
 //
@@ -17,22 +16,21 @@
 //   * The 5 A gate is the float OVERFLOW of d2: the records carry differences scaled by lambda = 2^64 / cut, so
 //     U = dx^2 + dy^2 + dz^2 = d2 2^128 / cut2 rounds to +inf exactly when the pair is outside the gate (threshold good to 3e-8;
 //     tests/test_gate_scheme_cpu.py restates the arithmetic).  r = U w with w = 1 / (sigma lambda)^2 (inf stays inf) and the
-//     minimum is an unpredicated FMNMX / FMNMX3 -- no compare, no predicate.  w is a denormal for sigma > 2.5 A
+//     minimum is an unpredicated FMNMX -- no compare, no predicate.  w is a denormal for sigma > 2.5 A
 //     (cut2 / sigma^2 < 4): FMUL handles denormals at full rate; w then keeps 21 + log2(cut2 / sigma^2) bits.
-//   * The FMA-pipe work runs on PACKED float32 pairs (fma.rn.f32x2 / mul.rn.f32x2, SASS FFMA2 / FMUL2, sm_100): (dy, dz), their
-//     squares, U and r of the four voxels take 7 issue slots per candidate; the epilogue evaluates two values per instruction.
+//   * Per candidate a lane evaluates (dy, dz), their squares and sum once, then U and r of its four voxels: 13 FMA-pipe
+//     instructions; the products and the sum are rounded on their own (no contraction), so r does not depend on the compiler.
 //   * Pairs whose d2 lies within 2e-6 (relative) of the gate -- where float32 could decide differently from the reference's
 //     float64 -- are found by a per-atom pre-pass (occ_band_kernel: the two lattice crossings of every (y, z) row of the
 //     cutoff sphere) and their voxels are recomputed in float64 with the reference's operation order by occ_fix_*_kernel.
-//   * Persistent CTAs (6 x 148 x 4 warps, 80 registers) pull (x, y, 4 z-blocks) items from an atomic queue.  The record pass
+//   * Persistent CTAs (5 per SM x 4 warps, 96 registers) pull (x, y, 4 z-blocks) items from an atomic queue.  The record pass
 //     gathers the per-atom data with cp.async straight into the candidates' sorted slots.  Results are staged in shared
 //     memory in the output layout; a block of a dense uniform batch leaves as ONE TMA tensor store (cp.async.bulk.tensor.4d,
 //     SASS UTMASTG; 4-D tensor map built per call), other outputs as cp.async.bulk row copies (UBLKCP); blocks without any
 //     atom in reach (~65 %) are copies from a zeroed shared-memory tile, no math.
-//   Measured and dropped in v10 (C3, ms per 256 pockets): a queue that runs two items ahead (0.735 -> 0.757: the second decode
-//   costs more issue slots than the latency it hides); peeling the first candidate of a run (0.758 -> 0.776); requesting the
-//   next z block's list words during the epilogue (0.689 -> 0.695, the extra live registers spill); 7 CTAs x 72 registers
-//   (0.699); 160 / 192 candidates per round (0.717 / 0.692); 2 z blocks per item (0.714).
+//   Tried and dropped: a queue that runs two items ahead (the second decode costs more issue slots than the latency it
+//   hides); peeling the first candidate of a run; requesting the next z block's list words during the epilogue (the extra
+//   live registers spill); 7 CTAs x 72 registers; 160 / 192 candidates per round; 2 z blocks per item.
 #pragma once
 
 namespace mkb {
@@ -47,7 +45,7 @@ constexpr int R_CAP = MKB_R_CAP;  // candidates per round (the 4 KB output stage
 #endif
 constexpr int R_WARPS = MKB_R_WARPS;
 #ifndef MKB_R_MIN_CTAS
-#define MKB_R_MIN_CTAS 6         // 6 x 4 warps with 80 registers
+#define MKB_R_MIN_CTAS 5         // 5 x 4 warps with 96 registers: at 6 x 80 the sm_90a build spills (4 % slower on an H100 SXM, 700 W)
 #endif
 #ifndef MKB_R_ZC
 #define MKB_R_ZC 4               // consecutive z blocks per queue item
@@ -70,7 +68,7 @@ struct RunParams {
     float *out;
     const long long *item_base;  // [B + 1]: first queue item of every grid (item = 4 x 4 voxels in x, y and R_ZC blocks in z)
     unsigned item0;              // first item of this launch's chunk of grids (queue ids are chunk-local)
-    int zc;                      // z blocks per item: R_ZC, or fewer when the batch has too few items to balance 4144 warps
+    int zc;                      // z blocks per item: R_ZC, or fewer when the batch has too few items to balance the resident warps
     unsigned *queue;
     unsigned total_items;
     int cmajor;                  // MKB_OCC_LAYOUT_CXYZ: grid stored [C][nx][ny][nz]; plain 32-byte-segment stores instead of TMA rows
@@ -166,7 +164,7 @@ __global__ void __launch_bounds__(128) occ_prep_kernel(const float *__restrict__
 }
 
 // second pass: the same walk appends (item, mask | multi << 8) to the lists; blk_count counts down to zero.  (Keeping the
-// slots of the first pass instead -- no atomics here -- was slower: 178 + 154 us against 95 + 144 us per 256 pockets.)
+// slots of the first pass instead -- no atomics here -- was slower.)
 __global__ void __launch_bounds__(128) occ_blk_fill_kernel(const GridDev *__restrict__ grids, int B, long long it0, long long n_items,
                                                            const float4 *__restrict__ rec_pos, const uint4 *__restrict__ rec_tag,
                                                            unsigned *__restrict__ blk_count, const unsigned *__restrict__ blk_start,
@@ -216,47 +214,6 @@ __device__ __forceinline__ float4 lds_rec4(unsigned a) {
     asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
     return v;
 }
-// packed float32 pairs (sm_100): a 64-bit register holds (lo, hi)
-typedef unsigned long long f2_t;
-__device__ __forceinline__ f2_t f2_pack(float lo, float hi) {
-    f2_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void f2_unpack(f2_t v, float &lo, float &hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f2_t f2_fma(f2_t a, f2_t b, f2_t c) {
-    f2_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-__device__ __forceinline__ f2_t f2_mul(f2_t a, f2_t b) {
-    f2_t r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-// occ_value() of two values at once: the same operations, each rounded as in the scalar form (identical results)
-__device__ __forceinline__ void occ_value_x2(float &x, float &y) {
-    const f2_t q = f2_pack(rcp_approx(x), rcp_approx(y));
-    const f2_t q3 = f2_mul(f2_mul(q, q), q);
-    const f2_t t = f2_mul(q3, q3);
-    f2_t s = f2_fma(t, f2_pack(-1.0f / 720.0f, -1.0f / 720.0f), f2_pack(1.0f / 120.0f, 1.0f / 120.0f));
-    s = f2_fma(t, s, f2_pack(-1.0f / 24.0f, -1.0f / 24.0f));
-    s = f2_fma(t, s, f2_pack(1.0f / 6.0f, 1.0f / 6.0f));
-    s = f2_fma(t, s, f2_pack(-0.5f, -0.5f));
-    s = f2_fma(t, s, f2_pack(1.0f, 1.0f));
-    s = f2_mul(s, t);
-    float e0, e1, t0, t1, s0, s1;
-    f2_unpack(f2_mul(t, f2_pack(-1.4426950408889634f, -1.4426950408889634f)), e0, e1);
-    f2_unpack(t, t0, t1);
-    f2_unpack(s, s0, s1);
-    x = t0 < 0.25f ? s0 : 1.0f - ex2_approx(e0);
-    y = t1 < 0.25f ? s1 : 1.0f - ex2_approx(e1);
-}
-// one LDS.128 as two packed pairs; volatile for the same reason as lds_rec4
-__device__ __forceinline__ void lds_2x64(unsigned a, f2_t &lo, f2_t &hi) {
-    asm volatile("ld.shared.v2.b64 {%0, %1}, [%2];" : "=l"(lo), "=l"(hi) : "r"(a));
-}
-
 __device__ __forceinline__ void cp_async16(unsigned dst_smem, const void *src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst_smem), "l"(src) : "memory");
 }
@@ -304,7 +261,7 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
     bool pending = false;  // lanes 0..15: bulk copies still reading the stage
     // lambda = 2^64 / cut (voxel units): d2 == cut2 lands on 2^128, the float overflow threshold
     // The FLOAT is the root value and the double its exact image: with lamf = (float)lam ptxas kept only the double and
-    // re-converted it (F2F.F32.F64, a slow-pipe instruction the first FFMA2 then waits for) at the head of EVERY hot-loop trip.
+    // re-converted it (F2F.F32.F64, a slow-pipe instruction the first FFMA then waits for) at the head of EVERY hot-loop trip.
     // Atoms and voxels are scaled by the same number this way; cwf = 2^64 / lambda (= cut up to 6e-8) keeps r = U w exact.
     float lamf = UNIFORM ? (float)(18446744073709551616.0 / sqrt((double)p.u.cut2v)) : 0.0f;
     asm volatile("mov.b32 %0, %0;" : "+f"(lamf));
@@ -545,16 +502,13 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
 #define MKB_RUN_R2(D, Y, R)                                                                       \
     float R##0, R##1, R##2, R##3;                                                                 \
     {                                                                                             \
-        const f2_t dyz = f2_fma(fyz, lam2, f2_pack(Y.x, Y.y));                                    \
-        float sl_, sh_;                                                                           \
-        f2_unpack(f2_mul(dyz, dyz), sl_, sh_);                                                    \
-        const float s2_ = sl_ + sh_;                                                              \
-        const f2_t ss_ = f2_pack(s2_, s2_), ww_ = f2_pack(Y.z, Y.z);                              \
-        const f2_t d01_ = f2_pack(D.x, D.y), d23_ = f2_pack(D.z, D.w);                            \
-        f2_unpack(f2_mul(f2_fma(d01_, d01_, ss_), ww_), R##0, R##1);                              \
-        f2_unpack(f2_mul(f2_fma(d23_, d23_, ss_), ww_), R##2, R##3);                              \
+        const float dy_ = fmaf(fy, lamf, Y.x), dz_ = fmaf(fz, lamf, Y.y);                         \
+        const float s2_ = __fadd_rn(__fmul_rn(dy_, dy_), __fmul_rn(dz_, dz_));                    \
+        R##0 = __fmul_rn(fmaf(D.x, D.x, s2_), Y.z);                                               \
+        R##1 = __fmul_rn(fmaf(D.y, D.y, s2_), Y.z);                                               \
+        R##2 = __fmul_rn(fmaf(D.z, D.z, s2_), Y.z);                                               \
+        R##3 = __fmul_rn(fmaf(D.w, D.w, s2_), Y.z);                                               \
     }
-                    const f2_t fyz = f2_pack(fy, fz), lam2 = f2_pack(lamf, lamf);
                     float4 a = MKB_LDREC(0), ya = MKB_LDRECY(0);
                     int i = 1;  // next record to load; i == np reads past the list (inside this warp's buffer), never used
                     float M0 = INF, M1 = INF, M2 = INF, M3 = INF;
@@ -635,13 +589,8 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
                 const float LIVE = 0.5f * R_GATE_HUGE;  // r of a voxel-channel no atom reached: +inf
                 const bool live = fminf(fminf(v.x, v.y), fminf(v.z, v.w)) < LIVE;
                 if (__any_sync(0xffffffffu, live)) {
-#if MKB_VALUE_SHORT
-                    occ_value_x2(v.x, v.y);
-                    occ_value_x2(v.z, v.w);
-#else
                     v.x = occ_value(rcp_approx(v.x)); v.y = occ_value(rcp_approx(v.y));
                     v.z = occ_value(rcp_approx(v.z)); v.w = occ_value(rcp_approx(v.w));
-#endif
                 } else {
                     v = make_float4(0.f, 0.f, 0.f, 0.f);
                 }

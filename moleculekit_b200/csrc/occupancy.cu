@@ -1,4 +1,4 @@
-// occupancy.cu -- K1/K1b/K2: voxel occupancy for sm_100a.
+// occupancy.cu -- K1/K1b/K2: voxel occupancy for sm_90a (H100).
 //
 // Replaces moleculekit/occupancy_utils/occupancy_utils.pyx:34-61 (calculate_occupancy) and the grid-centre
 // materialisation of moleculekit/tools/voxeldescriptors.py:125-132,197-248 on the device.
@@ -68,7 +68,7 @@ __device__ __forceinline__ float ex2_approx(float x) {
 }
 
 #ifndef MKB_VALUE_SHORT
-#define MKB_VALUE_SHORT 1  // measured: -0.8 % of the fill kernel
+#define MKB_VALUE_SHORT 1
 #endif
 // 1 - exp(-q^6), q = sigma^2/d2  (== 1 - exp(-(sigma/r)^12), occupancy_utils.pyx:57-60), relative error ~1e-6.
 __device__ __forceinline__ float occ_value(float q) {
@@ -1109,19 +1109,18 @@ constexpr int V_PCAP = MKB_V_PCAP;   // block candidates per round
 constexpr int V_QCAP = MKB_V_QCAP;   // sub-block candidates per round
 constexpr int V_QSTRIDE = V_QCAP + 2;  // + one sentinel slot for the software-pipelined loop
 #ifndef MKB_V_UNROLL2
-#define MKB_V_UNROLL2 0  // two candidates per trip: 2.19 vs 2.03 ms (spills at 72 registers)
+#define MKB_V_UNROLL2 0  // two candidates per trip (spills at 72 registers)
 #endif
 #ifndef MKB_V_WARPS
-#define MKB_V_WARPS 1    // warps (= blocks) per CTA. A CTA holds its registers until its slowest warp retires: 4 -> 2.03 ms, 2 -> 1.87, 1 -> 1.85
+#define MKB_V_WARPS 1    // warps (= blocks) per CTA. A CTA holds its registers until its slowest warp retires
 #endif
 constexpr int V_WARPS = MKB_V_WARPS;
 #ifndef MKB_V_ZPER
-#define MKB_V_ZPER 1     // consecutive z blocks walked by one warp: 1 -> 1.86 ms, 2 -> 2.08, 4 -> 1.93, 8 -> 1.99 (longer-lived CTAs balance worse)
+#define MKB_V_ZPER 1     // consecutive z blocks walked by one warp (longer-lived CTAs balance worse)
 #endif
 constexpr int V_ZPER = MKB_V_ZPER;
-// (a software-pipelined variant that loaded the next candidate ahead of the math gave 2.32 vs 2.30 ms and cost registers)
 #ifndef MKB_V_MIN_CTAS
-#define MKB_V_MIN_CTAS 7  // 72 registers: measured 2.09 ms; 6 CTAs (80 regs) 2.30 ms, 8 CTAs (64 regs, spills) 2.40 ms
+#define MKB_V_MIN_CTAS 7  // 72 registers; at 8 CTAs (64 registers) the kernel spills
 #endif
 
 __global__ void occ_block_total_v_kernel(const GridDev *__restrict__ grids, const unsigned *__restrict__ cell_start,
@@ -1605,8 +1604,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         if (!(grids[b].voxelsize > 0.0)) break;  // reported below
         const int cv = (int)std::ceil(CUTOFF_A / grids[b].voxelsize);
         // very fine grids: the halo of a block spans more cell rows than a warp keeps (cutoff > 11 voxels) -> tile kernel.
-        // (Up to v5 the tile kernel also took every cutoff > 7 voxels: 0.66 ms vs 0.86 ms on 0.5 A grids; the 64-voxel
-        // block kernel now does those in 0.63 ms.  MKB_OCC_WARP32=1 restores the old rule together with the old kernel.)
+        // (MKB_OCC_WARP32=1 restores the older rule -- the tile kernel for every cutoff > 7 voxels -- and the older kernel.)
         const bool old_rule = getenv("MKB_OCC_WARP32") != nullptr && cv > 7 && !force_warp;
         if (variant == 0 && (old_rule || ((1 + 2 * cv) / 4 + 1) * ((3 + 2 * cv) / 4 + 1) > W_ROWS)) variant = 1;
         if (variant == 1 && ((TILE - 1 + 2 * cv) / TILE + 1) * ((TILE - 1 + 2 * cv) / TILE + 1) > 128) variant = 2;
@@ -1671,9 +1669,8 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
                     !getenv("MKB_OCC_V6") && !force_warp && !getenv("MKB_OCC_WARP32");
     // The batch can be cut into chunks of grids (MKB_OCC_CHUNKS=n): the list build of chunk c + 1 then runs on a side stream
     // beside the fill kernel of chunk c.  Chunk c owns the slots [blk_off[c], blk_off[c + 1]) of blk_count / blk_start (its
-    // blocks + 1: every chunk has its own exclusive scan) and the entries from ent_off[c] on.  Measured on C3 (256 pockets):
-    // 1 chunk 1.38 ms per step, 2 chunks 1.43, 4 chunks 1.49, 8 chunks 1.68 (also with 6 or 5 fill CTAs per SM): the list
-    // build does not hide behind the persistent fill kernel and every extra launch adds a tail, so the default is ONE chunk.
+    // blocks + 1: every chunk has its own exclusive scan) and the entries from ent_off[c] on.  The list build does not
+    // hide behind the persistent fill kernel and every extra launch adds a tail, so the default is ONE chunk.
     int n_chunks = 1;
     std::vector<int> cgrid;                // [n_chunks + 1] first grid of every chunk
     std::vector<long long> blk_off, ent_off, item_off, atom_item_off, ibase;
@@ -1933,7 +1930,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
     fp.cmajor = (flags & MKB_OCC_LAYOUT_CXYZ) ? 1 : 0;
     fp.vec_ok = (C == 8 && ((uintptr_t)out % 16 == 0) && !fp.cmajor) ? 1 : 0;
     fp.txp_shift = 0;
-    // opt-in (MKB_OCC_BULK_STORE=1): measured 21 % slower in this non-persistent kernel because the CTA has to wait for
+    // opt-in (MKB_OCC_BULK_STORE=1): slower in this non-persistent kernel because the CTA has to wait for
     // the asynchronous smem read before it may retire; kept for the persistent variant (DESIGN.md section 6)
     fp.bulk_store = (fp.vec_ok && !(flags & MKB_OCC_ACCUMULATE) && getenv("MKB_OCC_BULK_STORE")) ? 1 : 0;
 

@@ -1,4 +1,4 @@
-// rings.cu -- K13: ring-based interaction detectors over a trajectory for sm_100a.
+// rings.cu -- K13: ring-based interaction detectors over a trajectory for sm_90a (H100).
 //
 // Replaces pipi.calculate (moleculekit/interactions/pipi/pipi.pyx:86-185, mode 0), cationpi.calculate
 // (interactions/cationpi/cationpi.pyx:91-173, mode 1) and sigmahole.calculate (interactions/sigmahole/sigmahole.pyx:91-174,

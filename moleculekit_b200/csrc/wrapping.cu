@@ -1,4 +1,4 @@
-// wrapping.cu -- K9 (SURVEY 8f row 4): orthorhombic periodic wrapping of bonded groups for sm_100a.
+// wrapping.cu -- K9 (SURVEY 8f row 4): orthorhombic periodic wrapping of bonded groups for sm_90a (H100).
 //
 // Replaces wrap_box (moleculekit/wrapping/wrapping.pyx:91-144), the loop Molecule.wrap runs for rectangular cells
 // (moleculekit/molecule.py:2077).  Per frame the reference (1) takes the box centre as the running mean of the
@@ -696,7 +696,7 @@ extern "C" int mkb_wrap_box(mkb_handle_t h, void *stream, const mkb_traj *t, con
     if (t->frame_stride < F || t->frame_stride_box < F) return fail(h, MKB_ERR_BAD_ARG, "frame stride < n_frames");
     const long long nchunks = cdiv(F, 32);
     const long long small_blocks = cdiv(n_ranges * F, WRAP_THREADS);
-    if (small_blocks + 4 * 148 >= (1ll << 31) || nchunks >= (1ll << 31))
+    if (small_blocks + 4ll * h->sm_count >= (1ll << 31) || nchunks >= (1ll << 31))
         return fail(h, MKB_ERR_BAD_ARG, "groups x frames too large for one launch");
     float *centre = nullptr;
     unsigned *long_list = nullptr, *n_long = nullptr;
@@ -751,7 +751,7 @@ extern "C" int mkb_wrap_triclinic(mkb_handle_t h, void *stream, const mkb_traj *
     if (t->frame_stride < F || bv_frame_stride < F) return fail(h, MKB_ERR_BAD_ARG, "frame stride < n_frames");
     const long long nchunks = cdiv(F, 32);
     const long long small_blocks = cdiv(n_ranges * F, WRAP_THREADS);
-    if (small_blocks + 4 * 148 >= (1ll << 31) || nchunks >= (1ll << 31) || cdiv(N * 3 * F, 256) >= (1ll << 31))
+    if (small_blocks + 4ll * h->sm_count >= (1ll << 31) || nchunks >= (1ll << 31) || cdiv(N * 3 * F, 256) >= (1ll << 31))
         return fail(h, MKB_ERR_BAD_ARG, "atoms x frames too large for one launch");
     // scratch: centre [3][F] | box_middle [3][F] | ntric [F] | err in S_COM; the frame table in S_SORT_PX
     float *fbuf = nullptr;

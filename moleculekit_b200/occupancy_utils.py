@@ -183,7 +183,7 @@ def wait_index(device) -> None:
 def default_host_threads() -> int:
     """Host threads for the compact-transfer expansion: the CPUs this process may use, shared fairly between the ranks of a
     one-process-per-GPU job on this host (torchrun's LOCAL_WORLD_SIZE), at most 32 -- beyond that the expansion is bound
-    by memory bandwidth, and 8 ranks x 32 threads oversubscribed a 128-thread host (80 ms instead of 25 ms per step).
+    by memory bandwidth, and 8 ranks x 32 threads oversubscribe a 128-thread host.
     ``MKB_HOST_THREADS`` overrides."""
     import os
 

@@ -1,7 +1,7 @@
 """Drop-in for ``moleculekit.projections.metricdistance`` (MetricDistance / MetricSelfDistance).
 
 Constructor arguments, defaults, output shapes / dtypes, error messages and ``getMapping`` follow
-moleculekit/projections/metricdistance.py:19-364; ``project`` runs on the B200 through libmkb200 (K3 dense
+moleculekit/projections/metricdistance.py:19-364; ``project`` runs on the GPU through libmkb200 (K3 dense
 distances / K5 group reductions, post-ops fused).  ``mol`` is duck-typed: a moleculekit ``Molecule`` or
 :class:`moleculekit_b200.molecule_lite.MolLite` (needs coords, box, chain, resid, resname, name, element,
 numAtoms, numFrames, atomselect).

@@ -51,7 +51,7 @@ def balanced_partition(costs: Sequence[float], world: int) -> np.ndarray:
 def bind_to_gpu_numa(index: int):
     """Pin this process to the CPUs next to GPU ``index`` (NVML affinity mask).  Call it before the first pinned buffer is
     allocated (``tools.voxeldescriptors.pinned_array``), so the page-locked memory is first touched on the GPU's NUMA node:
-    the 256-pocket batch end to end takes 20 ms with the result on the GPU's node and 37 ms on the other socket.
+    a result on the other socket makes every device-to-host copy cross the socket link.
     Returns a one-line description of what was done ("unbound ..." when NVML or the affinity call is unavailable)."""
     try:
         import pynvml

@@ -1,7 +1,7 @@
 """Drop-in for the voxelisation entry points of ``moleculekit.tools.voxeldescriptors``.
 
 ``getCenters`` / ``getVoxelDescriptors`` keep the reference's signatures, defaults, return arity and error
-messages (moleculekit/tools/voxeldescriptors.py:197-203,251-264,345-360); the occupancy fill runs on the B200
+messages (moleculekit/tools/voxeldescriptors.py:197-203,251-264,345-360); the occupancy fill runs on the GPU
 through libmkb200 (no CPU path).  ``getVoxelDescriptorsBatch`` is the batched form the hardware wants: many
 molecules / pockets per launch, optionally left on the device.
 
@@ -154,7 +154,7 @@ def getChannels(mol, aromaticNitrogen: bool = False, version: int = 2, validityc
         from moleculekit.tools.voxeldescriptors import getChannels as _ref_getChannels  # type: ignore
     except Exception as e:  # pragma: no cover - depends on the environment
         raise RuntimeError(
-            "Default channels need moleculekit's atom typing (getChannels), which is outside the B200 hot path. "
+            "Default channels need moleculekit's atom typing (getChannels), which is outside the GPU hot path. "
             "Pass userchannels=(natoms, nchannels) bool/float array.") from e
     return _ref_getChannels(mol, aromaticNitrogen, version, validitychecks)
 
@@ -504,9 +504,8 @@ def getVoxelDescriptorsBatch(coords, channels, *, boxsize=None, centers=None, bu
     if transfer == "compact" and not compact_ok:
         raise ValueError("transfer='compact' needs 8 channels, the voxel-major layout and host float32 / float64 results")
     # "auto": the compact route pays a block-index round trip and a host-thread expansion; it wins once the dense copy
-    # is long enough to hide them (C3: 256 pockets 27 vs 40 ms, 32 pockets 7.2 vs 5.3 ms on one B200)
-    # and on a host shared by many ranks the expansion competes for the same memory bandwidth as the DMA it replaces
-    # (8 ranks x 256 pockets: 80 vs 58 ms), so "auto" keeps the dense copy there
+    # is long enough to hide them (large batches such as C3's 256 pockets, not 32), and on a host shared by many ranks the
+    # expansion competes for the same memory bandwidth as the DMA it replaces, so "auto" keeps the dense copy there
     if transfer == "auto" and (batch.total_voxels * batch.C * 4 < (512 << 20) or int(os.environ.get("LOCAL_WORLD_SIZE", "1")) > 2):
         compact_ok = False
     if compact_ok and transfer != "dense":

@@ -16,12 +16,12 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
     """Plain `pytest tests` on a host without a CUDA device (or without the built library) skips the gpu-marked tests
-    instead of failing in the first one; `-m gpu` on the B200 box runs them (there is no CPU fallback to fall into)."""
+    instead of failing in the first one; `-m gpu` on a GPU machine runs them (there is no CPU fallback to fall into)."""
     reason = None
     try:
         import torch

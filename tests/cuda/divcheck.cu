@@ -1,5 +1,5 @@
 // divcheck.cu -- device check that mkb::div_by(a, b, refined_rcp(b)) == __fdiv_rn(a, b) bit for bit.
-// Built and run by tests/test_wrapping_gpu.py on the GPU box:  nvcc -arch=sm_100a -I moleculekit_b200/csrc ...
+// Built and run by tests/test_wrapping_gpu.py on a GPU:  nvcc -arch=sm_90a -I moleculekit_b200/csrc ...
 // Divisors: every integer 1..2^17, plus 2^14 larger ones up to 2^31 (the running-mean divisor n + 1).  Numerators per
 // divisor: random bit patterns over the whole float range (incl. zeros, denormals, Inf, NaN -> the fallback branch),
 // and for random quotients q the neighbours of q*b (rounding-boundary stress).

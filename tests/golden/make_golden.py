@@ -1,20 +1,20 @@
 """Generate the committed golden fixtures in tests/golden/ from the REFERENCE itself.
 
-Runs only in the build container (needs /root/reference).  Two sources are used:
+Needs a moleculekit source checkout, named by MKB_REFERENCE_SRC.  Two sources are used:
 
- 1. the reference's own stored goldens under /root/reference/tests (3PTB_voxres_old.npy,
+ 1. the reference's own stored goldens under $MKB_REFERENCE_SRC/tests (3PTB_voxres_old.npy,
     metricdistance/{distances,mindistances,selfmindistance}.npy, inline constants of
     tests/test_metricdistance.py / tests/test_interactions.py), sliced/sparsified so they are small;
  2. outputs of the reference's compiled Cython kernels (oracle/_ref, built from the .pyx files in
     place by oracle/build_ref.py) on seeded inputs, for cases the reference has no stored golden for
     (arbitrary centres, multi-sigma atoms, ordered contact pairs, COM reductions, cdist/pdist).
 
-Reading PDB/XTC files needs the full reference Python package with its extensions built; as
-/root/reference is read-only that build lives in a scratch copy (SURVEY.md appendix A):
+Reading PDB/XTC files needs the full reference Python package with its extensions built; the checkout is only read,
+so that build lives in a scratch copy (SURVEY.md appendix A):
 
-    mkdir /tmp/refcopy && cd /tmp/refcopy && cp -r /root/reference/moleculekit /root/reference/setup.py . \
+    mkdir $TMP/refcopy && cd $TMP/refcopy && cp -r $MKB_REFERENCE_SRC/moleculekit $MKB_REFERENCE_SRC/setup.py . \
       && chmod -R u+w . && python setup.py build_ext --inplace
-    cd /root/repo && PYTHONPATH=/tmp/refcopy LOCAL_PDB_REPO=/root/reference/tests/pdb python tests/golden/make_golden.py
+    cd <this repository> && PYTHONPATH=$TMP/refcopy LOCAL_PDB_REPO=$MKB_REFERENCE_SRC/tests/pdb python tests/golden/make_golden.py
 
 The fixtures carry only numbers (coordinates, masks, outputs) -- no reference source.
 """
@@ -29,12 +29,12 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-REFT = "/root/reference/tests"
+REFT = os.path.join(os.environ.get("MKB_REFERENCE_SRC", ""), "tests")
 
 
 def scratch_copy(path: str) -> str:
     """The reference's XTC reader drops index-cache files (.name, .name.numframes) next to the trajectory it reads;
-    /root/reference must not be written to, so trajectories are read from a scratch copy."""
+    the checkout must not be written to, so trajectories are read from a scratch copy."""
     import shutil
     import tempfile
 
@@ -648,7 +648,7 @@ def main():
         wrapping_fixture()
         return
 
-    assert build_ref.build(), "oracle/_ref could not be built (is /root/reference present?)"
+    assert build_ref.build(), "oracle/_ref could not be built (is MKB_REFERENCE_SRC set?)"
     occ_ref, dist_ref = build_ref.load()[:2]
 
     from moleculekit.molecule import Molecule  # the reference (scratch build on PYTHONPATH)

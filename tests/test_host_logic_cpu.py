@@ -165,7 +165,7 @@ def test_ring_decision_intervals(tmp_path):
         pytest.skip("nvcc not available")
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     exe = str(tmp_path / "ringsets")
-    subprocess.run([nvcc, "-O2", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", f"-I{root}/include",
+    subprocess.run([nvcc, "-O2", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", f"-I{root}/include",
                     f"-I{root}/moleculekit_b200/csrc", os.path.join(root, "tests", "cuda", "ringsets.cu"), "-o", exe],
                    check=True, capture_output=True)
     r = subprocess.run([exe], capture_output=True, text=True)

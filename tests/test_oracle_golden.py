@@ -122,10 +122,10 @@ def test_dist_trajectory_fixture_golden(oracle, g_traj):
 
 
 def test_oracle_vs_live_reference(oracle, refmods):
-    """When oracle/_ref is present (it is in the build container and travels to the GPU box),
-    compare against the reference's own binaries on fresh random inputs."""
+    """When oracle/_ref is present (MKB_REFERENCE_SRC names a moleculekit source checkout), compare against the
+    reference's own binaries on fresh random inputs."""
     if refmods is None:
-        pytest.skip("oracle/_ref not built (no /root/reference here)")
+        pytest.skip("oracle/_ref not built (MKB_REFERENCE_SRC not set)")
     occ_ref, dist_ref = refmods[:2]
     rng = np.random.default_rng(5)
     for trial in range(3):
@@ -158,7 +158,7 @@ def _canonical(b):
 def test_bond_grid_search_golden(oracle, g_bonds):
     """Row a13: the reference's 15 csv goldens (tests/test_bondguesser.py:27-44), compared like the reference does
     (after calculateUniqueBonds).  The oracle's raw output ORDER was additionally checked identical to the reference's
-    bond_grid_search in the build container (tests/golden/make_golden.py asserts the reference reproduces the csv)."""
+    bond_grid_search when the fixture was made (tests/golden/make_golden.py asserts the reference reproduces the csv)."""
     from moleculekit_b200 import bondguesser as bgm  # host-only use: the radii table and name rule
 
     g = g_bonds

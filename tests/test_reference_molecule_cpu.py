@@ -1,142 +1,118 @@
-"""The drop-in wrappers fed with the REFERENCE's own ``Molecule`` (VERDICT r1 weak #9), CPU only.
+"""The host prologues of the drop-in projections against the reference's own outputs, CPU only.
 
-Runs in the build container, where /root/reference exists: the reference's pure-Python package is imported from there with
-its compiled kernels taken from oracle/_ref (the reference's .pyx compiled by oracle/build_ref.py), a real ``Molecule`` is
-read from the reference's test files, and the host prologues of ``MetricDistance.project`` / ``MetricSelfDistance`` -- string
-selections through ``mol.atomselect``, group building, ``digitize_chains``, the arguments that reach the kernel -- are
-compared with the reference's up to the kernel call (both kernels are replaced by recorders, nothing runs on a GPU).
-Skipped on the GPU box, where the reference tree does not exist.
+tests/golden/traj20.npz holds the reference's test system (tests/test_projections/trajectory: 4507 atoms, every 10th
+frame) with the reference's selection masks and the float32 outputs of the reference's own ``MetricDistance`` /
+``MetricSelfDistance.project`` and ``calculate_contacts`` on it (tests/golden/make_golden.py).  Here the GPU kernel behind
+our wrappers is replaced by the C oracle (oracle/mkb_oracle.c, pinned bit for bit to the reference's compiled kernels
+by tests/test_oracle_golden.py), so what is compared is what the host prologue hands to the kernel -- selections, chain ids,
+self-distance / periodic flags, groups, masses, reductions, the truncate / threshold post-ops -- and the outputs must be
+the reference's bit for bit.
 """
-import os
-import shutil
-import sys
-
 import numpy as np
 import pytest
 
-REF = "/root/reference"
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "moleculekit")), reason="reference tree not present")
-
-
-@pytest.fixture(scope="module")
-def refmol(tmp_path_factory):
-    sys.path.insert(0, ROOT)
-    from oracle import build_ref
-
-    if not build_ref.build(verbose=False):
-        pytest.skip("oracle/_ref could not be built")
-    names = list(build_ref.MODULES)
-    mods = dict(zip(names, build_ref.load()))
-    if REF not in sys.path:
-        sys.path.insert(0, REF)
-    import moleculekit
-
-    for name, m in mods.items():
-        sys.modules["moleculekit." + name] = m
-        setattr(moleculekit, name, m)
-    from moleculekit.molecule import Molecule
-
-    # the reference's XTC reader writes index caches next to the file it opens: work on a scratch copy
-    d = tmp_path_factory.mktemp("traj")
-    for f in ("filtered.pdb", "traj.xtc"):
-        shutil.copy(os.path.join(REF, "tests", "test_projections", "trajectory", f), d / f)
-    mol = Molecule(str(d / "filtered.pdb"))
-    mol.read(str(d / "traj.xtc"))
-    mol.dropFrames(keep=np.arange(0, mol.numFrames, 20))
-    return mol
+def _bits(a):
+    a = np.ascontiguousarray(a, dtype=np.float32)
+    b = a.view(np.uint32).copy()
+    b[np.isnan(a)] = 0x7FC00000
+    return b
 
 
-class _Recorder:
-    def __init__(self):
-        self.calls = []
-
-    def __call__(self, *args, **kw):
-        self.calls.append(args)
-        return args[-1] if len(args) and isinstance(args[-1], np.ndarray) else None
-
-
-def _capture_reference(monkeypatch, fn_name, build_and_project):
-    rec = _Recorder()
-    # the reference imports the kernel inside its function (util.py:23,99): patch the compiled module it imports from
-    monkeypatch.setattr(sys.modules["moleculekit.distance_utils"], fn_name, rec)
-    build_and_project()
-    assert len(rec.calls) == 1
-    return rec.calls[0]
-
-
-def _capture_ours(monkeypatch, fn_name, build_and_project):
+@pytest.fixture
+def refmol(g_traj, oracle, monkeypatch):
+    """A MolLite of the reference's test system whose distance kernels are the C oracle."""
     from moleculekit_b200 import distance_utils as du
+    from moleculekit_b200.molecule_lite import MolLite
 
-    rec = _Recorder()
+    def post(results, metric, truncate, threshold):  # projections/util.py:74-84,212-223 of the reference
+        if truncate is not None:
+            results[results > truncate] = truncate
+        return results <= threshold if metric == "contacts" else results
 
-    def wrapper(*args, **kw):
-        rec.calls.append(args)
-        out = args[-1] if isinstance(args[-1], np.ndarray) else None
-        return out
+    def dist_trajectory(coords, box, sel1, sel2, chains, selfdist, pbc, results, device=None, metric="distances",
+                        truncate=None, threshold=8.0, exact=True):
+        oracle.dist_trajectory(coords, box, sel1, sel2, chains, selfdist, pbc, results)
+        return post(results, metric, truncate, threshold)
 
-    monkeypatch.setattr(du, fn_name, wrapper)
-    build_and_project()
-    assert len(rec.calls) == 1
-    return rec.calls[0]
+    def dist_trajectory_reduction(coords, box, groups1, groups2, ch1, ch2, selfdist, pbc, masses, r1, r2, results,
+                                  device=None, metric="distances", truncate=None, threshold=8.0):
+        oracle.dist_trajectory_reduction(coords, box, groups1, groups2, ch1, ch2, selfdist, pbc, masses, r1, r2, results)
+        return post(results, metric, truncate, threshold)
+
+    def contacts_trajectory_arrays(coords, box, sel1, sel2, chains, selfdist, pbc, threshold, device=None):
+        per_frame = oracle.contacts_trajectory(coords, box, sel1, sel2, chains, selfdist, pbc, threshold)
+        off = np.concatenate([[0], np.cumsum([len(x) // 2 for x in per_frame])]).astype(np.int64)
+        pairs = np.array([v for x in per_frame for v in x], dtype=np.uint32).reshape(-1, 2)
+        return off, pairs
+
+    monkeypatch.setattr(du, "dist_trajectory", dist_trajectory)
+    monkeypatch.setattr(du, "dist_trajectory_reduction", dist_trajectory_reduction)
+    monkeypatch.setattr(du, "contacts_trajectory_arrays", contacts_trajectory_arrays)
+    g = g_traj
+    return MolLite(g["coords"], g["box"], element=g["element"], name=g["name"], resname=g["resname"], resid=g["resid"],
+                   chain=g["chain"], segid=g["segid"],
+                   named_selections={s: m for s, m in zip(g["sel_strings"].tolist(), g["sel_masks"])})
 
 
 @pytest.mark.parametrize("periodic", [None, "chains", "selections"])
-def test_metricdistance_prologue_with_reference_molecule(refmol, monkeypatch, periodic):
-    """MetricDistance(string selections) on the reference Molecule: sel masks, chain ids, selfdist / pbc flags and the
-    trajectory arrays that reach dist_trajectory are those of the reference (metricdistance.py:132-179, util.py:12-85)."""
-    from moleculekit.projections.metricdistance import MetricDistance as RefMD
-    from moleculekit_b200.projections.metricdistance import MetricDistance as OurMD
+def test_metricdistance_prologue_with_reference_molecule(refmol, g_traj, periodic):
+    """MetricDistance / calculate_contacts with string selections: selection indices, chain ids and the selfdist / pbc
+    flags reach the kernel as the reference's do (metricdistance.py:132-179, util.py:12-85, distance.py)."""
+    from moleculekit_b200.distance import calculate_contacts
+    from moleculekit_b200.projections.metricdistance import MetricDistance
 
-    sel1, sel2 = "protein and name CA and resid 10 to 40", "resname MOL and noh"
-    ref_args = _capture_reference(monkeypatch, "dist_trajectory",
-                                  lambda: RefMD(sel1, sel2, periodic=periodic, metric="distances").project(refmol))
-    our_args = _capture_ours(monkeypatch, "dist_trajectory",
-                             lambda: OurMD(sel1, sel2, periodic=periodic, metric="distances").project(refmol))
-    # (coords, box, sel1, sel2, digitized_chains, selfdist, pbc, results)
-    for k, (a, b) in enumerate(zip(ref_args[:7], our_args[:7])):
-        if isinstance(a, np.ndarray):
-            assert a.dtype == b.dtype and np.array_equal(a, b), f"argument {k} differs"
-        else:
-            assert bool(a) == bool(b), f"argument {k} differs"
-    assert ref_args[7].shape == our_args[7].shape and ref_args[7].dtype == our_args[7].dtype
-
-
-def test_selfdistance_and_mapping_with_reference_molecule(refmol, monkeypatch):
-    """MetricSelfDistance + groupsel="residue" + getMapping on the reference Molecule (metricdistance.py:244-364)."""
-    from moleculekit.projections.metricdistance import MetricSelfDistance as RefSD
-    from moleculekit_b200.projections.metricdistance import MetricSelfDistance as OurSD
-
-    sel = "protein and name CA and resid 5 to 30"
-    ref_args = _capture_reference(monkeypatch, "dist_trajectory", lambda: RefSD(sel, periodic=None).project(refmol))
-    our_args = _capture_ours(monkeypatch, "dist_trajectory", lambda: OurSD(sel, periodic=None).project(refmol))
-    for a, b in zip(ref_args[:7], our_args[:7]):
-        if isinstance(a, np.ndarray):
-            assert np.array_equal(a, b)
-        else:
-            assert bool(a) == bool(b)
-    rm = RefSD(sel, periodic=None, groupsel="residue").getMapping(refmol)
-    om = OurSD(sel, periodic=None, groupsel="residue").getMapping(refmol)
-    assert list(rm.columns) == list(om.columns) and len(rm) == len(om)
-    assert rm["description"].tolist() == om["description"].tolist()
-    assert [list(np.atleast_1d(x)) for x in rm["atomIndexes"]] == [list(np.atleast_1d(x)) for x in om["atomIndexes"]]
+    g = g_traj
+    masks = dict(zip(g["sel_strings"].tolist(), g["sel_masks"]))
+    ca, lig, noh = masks["protein and name CA"], masks["resname MOL and noh"], masks["protein and noh"]
+    if periodic == "selections":
+        d = MetricDistance("protein and name CA", "resname MOL and noh", metric="distances", periodic=periodic).project(refmol)
+        assert d.dtype == np.float32 and np.array_equal(_bits(d), _bits(g["ref_distances"]))
+        c = MetricDistance("protein and name CA", "resname MOL and noh", metric="contacts", threshold=8,
+                           periodic=periodic).project(refmol)
+        assert c.dtype == bool and np.array_equal(c, g["ref_distances"] <= np.float32(8))
+        cnt, pairs, got = g["ct_ca_lig_sel8_cnt"], g["ct_ca_lig_sel8_pairs"], calculate_contacts(refmol, ca, lig, periodic, 8)
+    elif periodic == "chains":
+        d = MetricDistance("protein and resid 1 to 20 and noh", "resname MOL and noh", periodic=periodic).project(refmol)
+        assert np.array_equal(_bits(d), _bits(g["ref_chains_distances"]))
+        cnt, pairs, got = g["ct_noh_lig_chains5_cnt"], g["ct_noh_lig_chains5_pairs"], calculate_contacts(refmol, noh, lig, periodic, 5)
+    else:
+        cnt, pairs, got = g["ct_ca_ca_none6_cnt"], g["ct_ca_ca_none6_pairs"], calculate_contacts(refmol, ca, ca, periodic, 6)
+    assert [len(x) for x in got] == cnt.tolist()
+    assert np.array_equal(np.concatenate(got).astype(np.uint32), pairs)
 
 
-def test_reduction_prologue_with_reference_molecule(refmol, monkeypatch):
-    """Residue groups against a ligand (get_reduced_distances, util.py:88-223): groups, group chain ids, masses, flags."""
-    from moleculekit.projections.metricdistance import MetricDistance as RefMD
-    from moleculekit_b200.projections.metricdistance import MetricDistance as OurMD
+def test_selfdistance_and_mapping_with_reference_molecule(refmol, g_traj):
+    """MetricSelfDistance + groupsel="residue" (metricdistance.py:244-364): the residue groups and the self-distance
+    column order give the reference's output, and the mapping has one row per column."""
+    from moleculekit_b200.projections.metricdistance import MetricDistance, MetricSelfDistance
 
-    kw = dict(periodic="selections", groupsel1="residue", groupsel2="all", metric="contacts", threshold=6)
-    sel1, sel2 = "protein and resid 10 to 25 and noh", "resname MOL and noh"
-    ref_args = _capture_reference(monkeypatch, "dist_trajectory_reduction", lambda: RefMD(sel1, sel2, **kw).project(refmol))
-    our_args = _capture_ours(monkeypatch, "dist_trajectory_reduction", lambda: OurMD(sel1, sel2, **kw).project(refmol))
-    # (coords, box, groups1, groups2, chains1, chains2, selfdist, pbc, masses, red1, red2, results)
-    assert np.array_equal(ref_args[0], our_args[0]) and np.array_equal(ref_args[1], our_args[1])
-    assert [list(g) for g in ref_args[2]] == [list(g) for g in our_args[2]]
-    assert [list(g) for g in ref_args[3]] == [list(g) for g in our_args[3]]
-    for k in (4, 5, 8):
-        assert np.array_equal(np.asarray(ref_args[k]), np.asarray(our_args[k])), k
-    for k in (6, 7, 9, 10):
-        assert int(ref_args[k]) == int(our_args[k]), k
+    sel = "protein and resid 1 to 50 and noh"
+    auto = MetricSelfDistance(sel, groupsel="residue").project(refmol)
+    assert auto.shape == (20, 1225) and np.array_equal(_bits(auto), _bits(g_traj["ref_selfmindistance"]))
+    manual = MetricDistance(sel, sel, periodic=None, groupsel1="residue", groupsel2="residue").project(refmol)
+    assert np.array_equal(_bits(manual), _bits(auto))
+    mp = MetricSelfDistance(sel, groupsel="residue").getMapping(refmol)
+    assert len(mp) == auto.shape[1]
+    resid = np.asarray(g_traj["resid"])
+    a, b = (np.atleast_1d(x) for x in mp["atomIndexes"].iloc[0])  # first column: the selection's first two residues
+    assert len(set(resid[a])) == 1 and len(set(resid[b])) == 1 and resid[a][0] < resid[b][0]
+
+
+def test_reduction_prologue_with_reference_molecule(refmol, g_traj):
+    """Residue groups against a ligand (get_reduced_distances, util.py:88-223): groups, group chain ids, masses and the
+    closest / com reductions give the reference's outputs."""
+    from moleculekit_b200.projections.metricdistance import MetricDistance
+
+    g = g_traj
+    kw = dict(groupsel1="residue", groupsel2="all")
+    d = MetricDistance("protein and noh", "resname MOL and noh", periodic="selections", **kw).project(refmol)
+    assert d.shape == (20, 277) and np.array_equal(_bits(d), _bits(g["ref_mindistances"]))
+    c = MetricDistance("protein and noh", "resname MOL and noh", periodic="selections", metric="contacts", threshold=6,
+                       **kw).project(refmol)
+    assert np.array_equal(c, g["ref_mindistances"] <= np.float32(6))
+    b = "protein and resid 1 to 50 and noh"
+    cc = MetricDistance(b, "resname MOL and noh", "selections", groupreduce1="com", groupreduce2="com", **kw).project(refmol)
+    assert np.array_equal(_bits(cc), _bits(g["ref_com_com"]))
+    cl = MetricDistance(b, "resname MOL and noh", "selections", groupreduce1="com", groupreduce2="closest", **kw).project(refmol)
+    assert np.array_equal(_bits(cl), _bits(g["ref_com_closest"]))
