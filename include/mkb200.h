@@ -359,6 +359,37 @@ int mkb_rmsd(mkb_handle_t h, void *stream, const mkb_traj *t, const uint32_t *se
              const uint32_t *refsel, int64_t n_sel, const uint32_t *frames, int64_t n_frames, const double *records,
              float *out);
 
+/* K15: aligned coordinate features and per-atom fluctuations, replace the host gather of MetricCoordinate
+ * (moleculekit/projections/metriccoordinate.py) and the squared deviations of MetricFluctuation
+ * (moleculekit/projections/metricfluctuation.py).  All pointers except the mkb_traj struct are device pointers.  sel
+ * [n_sel] uint32 = the selected atoms of t in output order; n_sel == 0 is MKB_ERR_BAD_ARG.  frames [n_frames] uint32 = the
+ * listed frames of t (NULL = every frame, n_frames ignored); item k of the list is frame frames[k] and output row k
+ * belongs to it.  records [n][16] float64 = the K14 fit records of mkb_align_fit, record k for item k (NULL = no
+ * transform).  The aligned coordinate c is fl32(R (x - p_bar) + q_bar) evaluated in float64: the bits mkb_align_apply
+ * writes in place.  The trajectory is not modified.  Index ranges of sel, frames and group_offsets are the caller's
+ * responsibility.
+ *
+ * coordinates:  out[k * ld_out + d * n_sel + i] float32 = c_d of atom sel[i] in item k (one row per listed frame, all X
+ *               of the selection, then all Y, then all Z); ld_out >= 3 n_sel, so a frame shard can write into the rows
+ *               of a larger matrix, and the row block into the columns of a wider one.
+ * coord_sums:   sums[i * 3 + d] float64 = sum over the listed frames of c_d of atom sel[i] (zero without frames), added in
+ *               list order within fixed chunks of 64 items and the chunks in order: the bits depend only on the
+ *               selection and the ordered frame list (a frame slice gives the bits of the same explicit list).
+ * fluctuation:  centre [n_sel][3] float64 = the point each selected atom deviates from (the mean, or a reference).
+ *               Without group_offsets: out[k * ld_out + i] float32 = fl32(sum_d (c_d - centre[i][d])^2), the sum in
+ *               float64 (no fused multiply-add, axis order); ld_out >= n_sel.  With group_offsets [n_groups + 1] int64
+ *               (0 = first, n_sel = last, nondecreasing; a group is the selection positions [off[g], off[g+1]), empty
+ *               groups give NaN): out[k * ld_out + g] = fl32(the float64 mean of the group's unrounded per-atom values,
+ *               added in selection order); ld_out >= n_groups.  c is recomputed from the trajectory, never read back.
+ * The handle's timing events (mkb_set_timing) bracket the kernels (main; prep is empty). */
+int mkb_coordinates(mkb_handle_t h, void *stream, const mkb_traj *t, const uint32_t *sel, int64_t n_sel,
+                    const uint32_t *frames, int64_t n_frames, const double *records, float *out, int64_t ld_out);
+int mkb_coord_sums(mkb_handle_t h, void *stream, const mkb_traj *t, const uint32_t *sel, int64_t n_sel,
+                   const uint32_t *frames, int64_t n_frames, const double *records, double *sums);
+int mkb_fluctuation(mkb_handle_t h, void *stream, const mkb_traj *t, const uint32_t *sel, int64_t n_sel,
+                    const uint32_t *frames, int64_t n_frames, const double *records, const double *centre,
+                    const int64_t *group_offsets, int64_t n_groups, float *out, int64_t ld_out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -41,7 +41,7 @@ EXPORTS = [
     "mkb_cdist", "mkb_pdist", "mkb_squareform", "mkb_collisions_count", "mkb_collisions_fill",
     "mkb_bonds_count", "mkb_bonds_fill", "mkb_shell_counts", "mkb_wrap_box", "mkb_within_distance", "mkb_xtc_decode",
     "mkb_wrap_triclinic", "mkb_hbonds_count", "mkb_hbonds_fill", "mkb_ring_pairs_count", "mkb_ring_pairs_fill",
-    "mkb_align_fit", "mkb_align_apply", "mkb_rmsd",
+    "mkb_align_fit", "mkb_align_apply", "mkb_rmsd", "mkb_coordinates", "mkb_coord_sums", "mkb_fluctuation",
 ]
 
 _lib = None
@@ -115,6 +115,9 @@ def load():
     lib.mkb_align_fit.argtypes = [vp, vp, tp, vp, tp, vp, i64, vp, i64, vp, vp]
     lib.mkb_align_apply.argtypes = [vp, vp, tp, vp, i64, vp, vp]
     lib.mkb_rmsd.argtypes = [vp, vp, tp, vp, tp, vp, i64, vp, i64, vp, vp]
+    lib.mkb_coordinates.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, vp, i64]
+    lib.mkb_coord_sums.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, vp]
+    lib.mkb_fluctuation.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, vp, vp, i64, vp, i64]
     for name in EXPORTS:
         if name in ("mkb_last_error", "mkb_launch_count", "mkb_version", "mkb_last_kernel", "mkb_occupancy_compact_blocks"):
             continue

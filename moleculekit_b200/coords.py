@@ -1,0 +1,106 @@
+"""Aligned coordinate features, frame sums and per-atom fluctuations on the GPU (K15).
+
+  coordinates_device    (n, 3k) float32 rows: the aligned coordinates of the selection, X block | Y block | Z block
+  coord_sums_device     (k, 3) float64 sums over the listed frames (the mean is the sum over the frame count)
+  fluctuation_device    (n, k) or (n, G) float32 squared deviations from a centre, per atom or averaged per group
+
+CUDA tensors in, stream-ordered, like :func:`moleculekit_b200.align.rmsd_device`: ``coords`` is the (N, 3, F) float32
+frame-minor trajectory (or a frame slice of one), ``sel`` / ``frames`` int32 CUDA tensors (``frames`` None = every
+frame; row k belongs to frame ``frames[k]``) and ``records`` the (n, 16) float64 fit records of
+:func:`~moleculekit_b200.align.superpose_device` (None = no transform).  An aligned coordinate has the bits
+:func:`~moleculekit_b200.align.apply_device` would write; the trajectory is never modified and the aligned trajectory
+never materialised.  No CPU fallback.
+"""
+from __future__ import annotations
+
+import ctypes as C
+
+import torch
+
+from . import _lib
+from .align import RECORD, _traj
+from .distance_utils import _ptr
+from .occupancy_utils import _stream_ptr
+
+
+def _check_records(records, n):
+    if records is not None:
+        assert records.dtype == torch.float64 and tuple(records.shape) == (n, RECORD) and records.is_contiguous()
+
+
+def _rows(out, n, width, dtype, dev):
+    """``out`` or a new (n, width) tensor; a given ``out`` may be a row / column slice of a larger matrix (unit column
+    stride, any row stride)."""
+    if out is None:
+        return torch.empty((n, width), dtype=dtype, device=dev)
+    assert out.dtype == dtype and out.device == dev and out.ndim == 2 and tuple(out.shape) == (n, width)
+    assert n <= 1 or width == 0 or out.stride(1) == 1, "out needs unit column stride"
+    return out
+
+
+def coordinates_device(coords, sel, records=None, frames=None, out=None):
+    """(n, 3k) float32: row r = the aligned coordinates of the ``sel`` atoms in listed frame r, all X of the selection in
+    selection order, then all Y, then all Z.  ``out`` (optional) receives them, e.g. a frame shard's rows of a whole
+    trajectory's matrix."""
+    dev = coords.device
+    k = int(sel.numel())
+    n = coords.shape[2] if frames is None else int(frames.numel())
+    _check_records(records, n)
+    out = _rows(out, n, 3 * k, torch.float32, dev)
+    if n == 0:  # an empty frame list has a NULL data pointer, which the library reads as "every frame"
+        return out
+    ld = max(out.stride(0) if n > 1 else 3 * k, 3 * k)
+    h = _lib.handle(dev.index)
+    t = _traj(coords)
+    with torch.cuda.device(dev):
+        rc = _lib.load().mkb_coordinates(h, _stream_ptr(dev), C.byref(t), _ptr(sel), k, _ptr(frames), n,
+                                         _ptr(records), _ptr(out), ld)
+    _lib.check(rc, h)
+    return out
+
+
+def coord_sums_device(coords, sel, records=None, frames=None):
+    """(k, 3) float64: per selected atom and axis, the sum over the listed frames of the aligned float32 coordinate.  The
+    summation order depends only on the selection and the ordered frame list (fixed chunks of 64 frames, added in
+    order), so repeated calls, a frame slice and the equivalent explicit list give the same bits."""
+    dev = coords.device
+    k = int(sel.numel())
+    n = coords.shape[2] if frames is None else int(frames.numel())
+    _check_records(records, n)
+    sums = torch.empty((k, 3), dtype=torch.float64, device=dev)
+    if n == 0:
+        return sums.zero_()
+    h = _lib.handle(dev.index)
+    t = _traj(coords)
+    with torch.cuda.device(dev):
+        rc = _lib.load().mkb_coord_sums(h, _stream_ptr(dev), C.byref(t), _ptr(sel), k, _ptr(frames), n,
+                                        _ptr(records), _ptr(sums))
+    _lib.check(rc, h)
+    return sums
+
+
+def fluctuation_device(coords, sel, centre, records=None, frames=None, groups=None, out=None):
+    """Per listed frame and selected atom, fl32(sum_d (c_d - centre_d)^2) evaluated in float64, c the aligned float32
+    coordinate and ``centre`` a (k, 3) float64 CUDA tensor (the mean or a reference structure): (n, k) float32.  With
+    ``groups`` (G + 1,) int64 offsets over selection positions (0 first, k last, nondecreasing, no empty group) the
+    result is (n, G): the float64 mean of each group's per-atom values, rounded once."""
+    dev = coords.device
+    k = int(sel.numel())
+    n = coords.shape[2] if frames is None else int(frames.numel())
+    _check_records(records, n)
+    assert centre.dtype == torch.float64 and tuple(centre.shape) == (k, 3) and centre.is_contiguous()
+    G = k
+    if groups is not None:
+        assert groups.dtype == torch.int64 and groups.ndim == 1 and groups.is_contiguous()
+        G = int(groups.numel()) - 1
+    out = _rows(out, n, G, torch.float32, dev)
+    if n == 0:
+        return out
+    ld = max(out.stride(0) if n > 1 else G, G)
+    h = _lib.handle(dev.index)
+    t = _traj(coords)
+    with torch.cuda.device(dev):
+        rc = _lib.load().mkb_fluctuation(h, _stream_ptr(dev), C.byref(t), _ptr(sel), k, _ptr(frames), n,
+                                         _ptr(records), _ptr(centre), _ptr(groups), G, _ptr(out), ld)
+    _lib.check(rc, h)
+    return out

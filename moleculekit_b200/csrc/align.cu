@@ -339,12 +339,8 @@ __global__ void __launch_bounds__(AL_THREADS) align_apply_kernel(float *__restri
     const long long item = 32ll * blockIdx.x + lane;
     if (item >= n || (status && status[item] != 0)) return;
     const long long f = frames ? (long long)frames[item] : item;
-    const double *r = rec + item * AL_REC;
     double R[9], pb[3], qb[3];
-#pragma unroll
-    for (int j = 0; j < 9; ++j) R[j] = r[j];
-#pragma unroll
-    for (int d = 0; d < 3; ++d) { pb[d] = r[9 + d]; qb[d] = r[12 + d]; }
+    fit_record_load(rec + item * AL_REC, R, pb, qb);
     float *base = coords + f;
     const long long step = (long long)gridDim.y * AL_WARPS;
     for (long long a0 = (long long)blockIdx.y * AL_WARPS + w; a0 < N; a0 += step * AL_BATCH) {
@@ -361,11 +357,10 @@ __global__ void __launch_bounds__(AL_THREADS) align_apply_kernel(float *__restri
         for (int u = 0; u < AL_BATCH; ++u) {
             const long long a = a0 + step * u;
             if (a < N) {
-                const double x0 = (double)x[u][0] - pb[0], x1 = (double)x[u][1] - pb[1], x2 = (double)x[u][2] - pb[2];
+                float y[3];
+                fit_transform(R, pb, qb, x[u][0], x[u][1], x[u][2], y);
 #pragma unroll
-                for (int d = 0; d < 3; ++d)
-                    base[(a * 3 + d) * fs] =
-                        __double2float_rn(fma(R[3 * d + 2], x2, fma(R[3 * d + 1], x1, R[3 * d] * x0)) + qb[d]);
+                for (int d = 0; d < 3; ++d) base[(a * 3 + d) * fs] = y[d];
             }
         }
     }

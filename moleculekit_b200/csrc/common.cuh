@@ -35,6 +35,7 @@ enum ScratchSlot {
     S_BLK_SLOTS,    // occupancy run kernel: the slot of every (atom, block) insertion
     S_ALIGN_PART,   // K14: per-(segment, frame) partial sums of the fit / RMSD
     S_ALIGN_REF,    // K14: the centred reference selection
+    S_COORD_PART,   // K15: per-(frame chunk, atom, axis) partial frame sums
     S_NSLOTS
 };
 
@@ -203,5 +204,23 @@ struct StreamOrder {
     } while (0)
 
 inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// K14 fit record [16] float64: R (3x3 row-major), p_bar (3), q_bar (3), pad
+__device__ __forceinline__ void fit_record_load(const double *r, double (&R)[9], double (&pb)[3], double (&qb)[3]) {
+#pragma unroll
+    for (int j = 0; j < 9; ++j) R[j] = r[j];
+#pragma unroll
+    for (int d = 0; d < 3; ++d) { pb[d] = r[9 + d]; qb[d] = r[12 + d]; }
+}
+
+// y = fl32(R (x - p_bar) + q_bar) evaluated in float64: the one definition of an aligned coordinate (K14 apply and the
+// K15 coordinate / frame-sum / fluctuation kernels), so the in-place and the gathered results cannot drift apart
+__device__ __forceinline__ void fit_transform(const double (&R)[9], const double (&pb)[3], const double (&qb)[3],
+                                              float x0f, float x1f, float x2f, float (&y)[3]) {
+    const double x0 = (double)x0f - pb[0], x1 = (double)x1f - pb[1], x2 = (double)x2f - pb[2];
+#pragma unroll
+    for (int d = 0; d < 3; ++d)
+        y[d] = __double2float_rn(fma(R[3 * d + 2], x2, fma(R[3 * d + 1], x1, R[3 * d] * x0)) + qb[d]);
+}
 
 }  // namespace mkb

@@ -148,7 +148,14 @@ def voxelize_sharded(coords, channels, *, boxsize=None, centers=None, buffer=0.0
 def project_sharded(projection, mol, *, gather: bool = True, group=None):
     """Project a trajectory with frames split across ranks (MetricDistance.project on each frame block).
 
-    Returns the (F, P) numpy array on every rank when gather=True, else this rank's rows and its (f0, f1)."""
+    Returns the (F, P) numpy array on every rank when gather=True, else this rank's rows and its (f0, f1).  Only
+    projections whose frames are independent shard this way: a MetricFluctuation without a reference (its centre is the
+    mean over all frames) raises ValueError, use :func:`fluctuation_sharded`."""
+    from .projections.metricfluctuation import MetricFluctuation
+
+    if isinstance(projection, MetricFluctuation) and projection._refmol is None:
+        raise ValueError("project_sharded would take each rank's mean over its own frames: a MetricFluctuation without "
+                         "refmol deviates from the mean over all frames, use sharding.fluctuation_sharded")
     world, rank = world_info(group)
     F = mol.numFrames
     off = partition(F, world)
@@ -164,6 +171,46 @@ def project_sharded(projection, mol, *, gather: bool = True, group=None):
     full = gather_rows(t, [int(off[r + 1] - off[r]) for r in range(world)], group=group)
     res = full.cpu().numpy()
     return res.astype(bool) if local.dtype == bool else res
+
+
+def fluctuation_sharded(metric, mol, *, gather: bool = True, group=None, compute_fn=None):
+    """MetricFluctuation.project with the frames split across ranks.  Without a reference every rank sums its frames'
+    (wrapped) coordinates (K15 frame sums), the ranks all_gather the (n, 3) float64 sums and add them in rank order (the
+    same bits on every rank, deterministic for a given world size), and each rank then computes its own frames'
+    deviations from that mean; with a reference the centre is the reference's and no collective is needed before the
+    deviations.  Returns the (F, n or R) numpy array on every rank when gather=True, else this rank's rows and its
+    (f0, f1).  ``compute_fn(metric, view, centre)`` returns the view's (n, 3) frame sums when ``centre`` is None and its
+    deviations from ``centre`` otherwise; it defaults to ``metric.frame_sums`` / ``metric.deviations`` (the gloo tests
+    pass a CPU stand-in)."""
+    if compute_fn is None:
+        def compute_fn(m, view, centre):
+            return m.frame_sums(view) if centre is None else m.deviations(view, centre)
+    world, rank = world_info(group)
+    F = mol.coords.shape[2]
+    off = partition(F, world)
+    f0, f1 = int(off[rank]), int(off[rank + 1])
+    view = _frame_view(mol, f0, f1)
+    dev = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
+    centre = metric.reference_centre(mol)
+    if centre is None:
+        sums = np.ascontiguousarray(compute_fn(metric, view, None), dtype=np.float64)
+        if world > 1:
+            t = torch.from_numpy(sums).to(dev)
+            parts = [torch.empty_like(t) for _ in range(world)]
+            dist.all_gather(parts, t, group=group)
+            total = parts[0].cpu().numpy().copy()
+            for p in parts[1:]:
+                total += p.cpu().numpy()
+            sums = total
+        centre = sums / F if F else sums
+    local = np.asarray(compute_fn(metric, view, centre))
+    if not gather:
+        return local, (f0, f1)
+    if world == 1:
+        return local
+    full = gather_rows(torch.from_numpy(np.ascontiguousarray(local)).to(dev),
+                       [int(off[r + 1] - off[r]) for r in range(world)], group=group)
+    return full.cpu().numpy()
 
 
 def wrap_sharded(mol, *, gather: bool = True, group=None, wrap_fn=None, **wrap_kwargs):
