@@ -139,10 +139,12 @@ __global__ void xtc_decode_kernel(const unsigned char *__restrict__ file, long l
         for (long long w = 0; w < 3 * natoms; ++w) emit(w, xtc_be_float(data + 4 * w));
         return;
     }
+    // Lattice arithmetic is modulo 2^32, as the format defines it: a range of 2^31 or more, or a run next to INT_MIN,
+    // overflows signed int, so sizes and sums are formed in unsigned and only the final coordinate is read as int.
     unsigned sizeint[3];
     int bitsizeint[3] = {0, 0, 0};
 #pragma unroll
-    for (int d = 0; d < 3; ++d) sizeint[d] = (unsigned)(fr.maxint[d] - fr.minint[d] + 1);
+    for (int d = 0; d < 3; ++d) sizeint[d] = (unsigned)fr.maxint[d] - (unsigned)fr.minint[d] + 1u;
     if (!sizeint[0] || !sizeint[1] || !sizeint[2]) { status[f] = -2; return; }
     int bitsize;
     if ((sizeint[0] | sizeint[1] | sizeint[2]) > 0xffffffu) {
@@ -173,7 +175,7 @@ __global__ void xtc_decode_kernel(const unsigned char *__restrict__ file, long l
         }
         ++i;
 #pragma unroll
-        for (int d = 0; d < 3; ++d) { cur[d] += fr.minint[d]; prev[d] = cur[d]; }
+        for (int d = 0; d < 3; ++d) { cur[d] = (int)((unsigned)cur[d] + (unsigned)fr.minint[d]); prev[d] = cur[d]; }
         int is_smaller = 0;
         if (b.take(1)) {
             run = (int)b.take(5);
@@ -187,7 +189,7 @@ __global__ void xtc_decode_kernel(const unsigned char *__restrict__ file, long l
                 b.take3(smallidx, sizesmall, sizesmall, s);
                 ++i;
 #pragma unroll
-                for (int d = 0; d < 3; ++d) s[d] += prev[d] - smallnum;
+                for (int d = 0; d < 3; ++d) s[d] = (int)((unsigned)s[d] + (unsigned)prev[d] - (unsigned)smallnum);
                 if (w + (k == 0 ? 6 : 3) > wmax) { status[f] = -4; return; }
                 if (k == 0) {  // the first atom of a run is written before the atom it was coded against
 #pragma unroll

@@ -565,7 +565,7 @@ EXPORT int oracle_xtc_decode_block(const uint8_t *data, int64_t nbytes, int64_t 
 {
     uint32_t sizeint[3], bitsizeint[3] = {0, 0, 0};
     for (int d = 0; d < 3; ++d) {
-        sizeint[d] = (uint32_t)(maxint[d] - minint[d] + 1);
+        sizeint[d] = (uint32_t)maxint[d] - (uint32_t)minint[d] + 1u;  /* modulo 2^32: ranges >= 2^31 overflow int */
         if (!sizeint[d]) return -2;
     }
     int bitsize;
@@ -592,7 +592,7 @@ EXPORT int oracle_xtc_decode_block(const uint8_t *data, int64_t nbytes, int64_t 
             xtc_take3(&b, bitsize, sizeint, cur);
         }
         ++i;
-        for (int d = 0; d < 3; ++d) { cur[d] += minint[d]; prev[d] = cur[d]; }
+        for (int d = 0; d < 3; ++d) { cur[d] = (int32_t)((uint32_t)cur[d] + (uint32_t)minint[d]); prev[d] = cur[d]; }
         int is_smaller = 0;
         if (xtc_take(&b, 1)) {
             run = (int)xtc_take(&b, 5);
@@ -605,7 +605,7 @@ EXPORT int oracle_xtc_decode_block(const uint8_t *data, int64_t nbytes, int64_t 
                 int32_t s[3];
                 xtc_take3(&b, smallidx, sizesmall, s);
                 ++i;
-                for (int d = 0; d < 3; ++d) s[d] += prev[d] - smallnum;
+                for (int d = 0; d < 3; ++d) s[d] = (int32_t)((uint32_t)s[d] + (uint32_t)prev[d] - (uint32_t)smallnum);
                 if (k == 0) {  /* the first atom of the run goes BEFORE the atom it was coded against */
                     if (w + 3 > natoms * 3) return -4;
                     for (int d = 0; d < 3; ++d) { out[w++] = (float)s[d] * inv_precision; prev[d] = s[d]; }
