@@ -390,6 +390,26 @@ int mkb_fluctuation(mkb_handle_t h, void *stream, const mkb_traj *t, const uint3
                     const uint32_t *frames, int64_t n_frames, const double *records, const double *centre,
                     const int64_t *group_offsets, int64_t n_groups, float *out, int64_t ld_out);
 
+/* K16: torsion angles, replace the per-dihedral loop of MetricDihedral (moleculekit/projections/metricdihedral.py over
+ * moleculekit.dihedral.dihedralAngle).  All pointers except the mkb_traj struct are device pointers.  quads [n_quads][4]
+ * int32 = atom rows of t (p0, p1, p2, p3 of each dihedral), 16-byte aligned; n_quads == 0 is MKB_ERR_BAD_ARG.  frames
+ * [n_frames] uint32 = the listed frames of t (NULL = every frame, n_frames ignored); item k of the list is frame
+ * frames[k] and output row k belongs to it.  Index ranges of quads and frames are the caller's responsibility.  The
+ * coordinates are used as given (no minimum image), and nothing about the trajectory's orientation is needed.
+ *
+ * Per (item, quadruple), in float64 from the float32 points: b0 = p0 - p1, b1 = p2 - p1, b2 = p3 - p2, u = b1 / |b1|,
+ * v = b0 - (b0.u) u, w = b2 - (b2.u) u, x = v.w, y = (u x v).w.  The sign is IUPAC's: looking along p1 -> p2 the angle
+ * is positive when p1-p0 turns clockwise onto p2-p3 (cis 0, trans +-pi).
+ *   sincos == 0:  out[k * ld_out + j] float32 = fl32(atan2(y, x)), radians; ld_out >= n_quads.
+ *   sincos == 1:  out[k * ld_out + 2 j] = fl32(y / hypot(x, y)) (sine), out[k * ld_out + 2 j + 1] = fl32(x / hypot(x, y))
+ *                 (cosine); ld_out >= 2 n_quads.
+ * A degenerate quadruple -- b0 x b1 or b1 x b2 exactly zero, each component a[i] b[j] - a[j] b[i] evaluated in float64
+ * without a fused multiply-add (p0, p1, p2 or p1, p2, p3 collinear in any orientation, or p1 == p2) -- gives angle 0 and
+ * (sin, cos) = (0, 1); a non-finite coordinate among the four points gives NaN.  ld_out lets a frame shard write into the rows of a
+ * larger matrix.  The handle's timing events (mkb_set_timing) bracket the kernel (main; prep is empty). */
+int mkb_dihedrals(mkb_handle_t h, void *stream, const mkb_traj *t, const int32_t *quads, int64_t n_quads,
+                  const uint32_t *frames, int64_t n_frames, int32_t sincos, float *out, int64_t ld_out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -42,6 +42,7 @@ EXPORTS = [
     "mkb_bonds_count", "mkb_bonds_fill", "mkb_shell_counts", "mkb_wrap_box", "mkb_within_distance", "mkb_xtc_decode",
     "mkb_wrap_triclinic", "mkb_hbonds_count", "mkb_hbonds_fill", "mkb_ring_pairs_count", "mkb_ring_pairs_fill",
     "mkb_align_fit", "mkb_align_apply", "mkb_rmsd", "mkb_coordinates", "mkb_coord_sums", "mkb_fluctuation",
+    "mkb_dihedrals",
 ]
 
 _lib = None
@@ -118,6 +119,7 @@ def load():
     lib.mkb_coordinates.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, vp, i64]
     lib.mkb_coord_sums.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, vp]
     lib.mkb_fluctuation.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, vp, vp, i64, vp, i64]
+    lib.mkb_dihedrals.argtypes = [vp, vp, tp, vp, i64, vp, i64, i32, vp, i64]
     for name in EXPORTS:
         if name in ("mkb_last_error", "mkb_launch_count", "mkb_version", "mkb_last_kernel", "mkb_occupancy_compact_blocks"):
             continue
