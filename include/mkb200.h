@@ -410,6 +410,34 @@ int mkb_fluctuation(mkb_handle_t h, void *stream, const mkb_traj *t, const uint3
 int mkb_dihedrals(mkb_handle_t h, void *stream, const mkb_traj *t, const int32_t *quads, int64_t n_quads,
                   const uint32_t *frames, int64_t n_frames, int32_t sincos, float *out, int64_t ld_out);
 
+/* K17: Shrake-Rupley solvent-accessible surface area, replaces mdtraj's per-frame asa_frame loop that moleculekit's
+ * MetricSasa calls.  All pointers except the mkb_traj struct are device pointers.  env [n_env] uint32 = atom rows of t
+ * that form the environment (the reference's filtersel); radii [n_env] float32 = radius plus probe in nm, finite and
+ * > 0; query [n_query] uint32 = positions in env of the atoms whose area is computed; sphere [n_sphere][3] float32 =
+ * unit sphere points, 1 <= n_sphere <= 65536.  frames [n_frames] uint32 = the listed frames of t (NULL = every frame,
+ * n_frames ignored); output row k belongs to item k.  Index ranges are the caller's responsibility.  No wrapping and no
+ * minimum image.
+ *
+ * Per item, every operation float32 and rounded on its own (no fused multiply-add): x_nm = fl(x / 10); env atom j is
+ * a neighbour of query atom i when j != i and fl(fl(fl(dx dx) + fl(dy dy)) + fl(dz dz)) < fl(fl(R_i + R_j)^2), dx =
+ * fl(x_i - x_j); sphere point s of i sits at p = fl(x_i + fl(R_i s)) and is buried when the same sum over fl(p - x_k)
+ * is < fl(R_k R_k) for some neighbour k; n_i = the points not buried; a_i = fl(fl(fl(c R_i) R_i) n_i) nm^2 with
+ * c = (float)(4 pi / n_sphere).  A non-finite coordinate takes part in no neighbour relation.
+ *   group_offsets NULL:  out[k * ld_out + q] = fl(a_q 100) (Angstrom^2); ld_out >= n_query.
+ *   group_offsets [n_groups + 1] int64 (query positions, non-decreasing, first 0, last n_query):
+ *                        out[k * ld_out + g] = fl(s 100), s = the a_q of group g added in order to a float32 zero;
+ *                        ld_out >= n_groups.
+ * status [1] int64, 8-byte aligned: -1 when no query atom has an env atom j != i with d2 < 1e-10 nm^2 (coincident
+ * atoms, where the reference exits), else (item << 32) | q of the first such item and query (smallest key).  The
+ * listed frames are processed in chunks of mkb_sasa_chunk_frames(n_env, n_query, n_groups) items (0 with groups
+ * absent means n_groups = 0), so scratch stays bounded.  The handle's timing events bracket the whole call (main; prep
+ * is empty). */
+int mkb_sasa(mkb_handle_t h, void *stream, const mkb_traj *t, const uint32_t *env, int64_t n_env, const float *radii,
+             const uint32_t *query, int64_t n_query, const int64_t *group_offsets, int64_t n_groups,
+             const float *sphere, int32_t n_sphere, const uint32_t *frames, int64_t n_frames, float *out,
+             int64_t ld_out, int64_t *status);
+int64_t mkb_sasa_chunk_frames(int64_t n_env, int64_t n_query, int64_t n_groups);
+
 #ifdef __cplusplus
 }
 #endif

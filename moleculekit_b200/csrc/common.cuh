@@ -36,6 +36,14 @@ enum ScratchSlot {
     S_ALIGN_PART,   // K14: per-(segment, frame) partial sums of the fit / RMSD
     S_ALIGN_REF,    // K14: the centred reference selection
     S_COORD_PART,   // K15: per-(frame chunk, atom, axis) partial frame sums
+    S_SASA_REC,     // K17: gathered (x, y, z, R) records of a frame chunk
+    S_SASA_SORTED,  // K17: the records sorted by cell bucket
+    S_SASA_ITEM,    // K17: (bucket, slot) of every record
+    S_SASA_SIDX,    // K17: environment index of every sorted record
+    S_SASA_COUNT,   // K17: atoms per bucket
+    S_SASA_START,   // K17: first sorted record of every bucket
+    S_SASA_MAXR,    // K17: largest radius
+    S_SASA_AREA,    // K17: per-atom areas before the group sums
     S_NSLOTS
 };
 
