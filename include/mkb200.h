@@ -438,6 +438,40 @@ int mkb_sasa(mkb_handle_t h, void *stream, const mkb_traj *t, const uint32_t *en
              int64_t ld_out, int64_t *status);
 int64_t mkb_sasa_chunk_frames(int64_t n_env, int64_t n_query, int64_t n_groups);
 
+/* K18: DSSP secondary structure, replaces mdtraj's compute_dssp (a port of DSSP 2.2.0) that moleculekit's
+ * MetricSecondaryStructure calls per frame.  All pointers except the mkb_traj struct are device pointers.  backbone
+ * [n_res][4] int32 = atom rows of t of the N, CA, C and O of every residue of the DSSP sequence (all chains
+ * concatenated, indexed 0..n_res-1), 1 <= n_res <= 2^28; flags [n_res] uint8: bit 0 = proline, bit 1 = the residue
+ * differs in chain or segid from the previous one.  frames [n_frames] uint32 = the listed frames of t (NULL = every
+ * frame, n_frames ignored); item k is frame frames[k].  Index ranges are the caller's responsibility.  No minimum image.
+ *
+ * Per item, everything in float64 from the float32 Angstrom coordinates, every operation rounded on its own (no fused
+ * multiply-add); dist(a, b) = sqrt((dx dx + dy dy) + dz dz), d = a - b.
+ *   breaks   between r and r + 1 when bit 1 of flags[r + 1] is set or dist(C_r, N_r+1) > 2.5 (a NaN distance is not a
+ *            break); NoChainBreak(a, b) = no break between consecutive residues of [a, b].
+ *   H        H_r = N_r + v / |v| per component, v = C_r-1 - O_r-1, when r is not proline, r > 0 and no break lies
+ *            between r - 1 and r; else H_r = N_r.
+ *   energy   E(d, a) for donor d (N-H) and acceptor a (C=O), evaluated when a != d, a != d - 1, d is not proline and
+ *            dist(CA_d, CA_a) < 9.0: -9.9 when one of dHO, dHC, dNC, dNO is < 0.5, else
+ *            ((K/dHO - K/dHC) + K/dNC) - K/dNO with K = -27.888; then E = round(E 1000) / 1000 (half away from zero)
+ *            and E = -9.9 where E < -9.9.  Each donor keeps two slots (partner, energy), initially (-1, 0.0), filled in
+ *            ascending acceptor order: E < slot0.E shifts slot 0 to slot 1 and takes slot 0, else E < slot1.E takes
+ *            slot 1 (the stable top two by (E, index) among E < 0).  TestBond(x, y) = a slot of x holds y with E < -0.5.
+ *   bend     residue i with i - 2, i + 2 in range and NoChainBreak(i - 2, i + 2): u = CA_i - CA_i-2,
+ *            w = CA_i+2 - CA_i, x = (u.u)(w.w), c = (u.w) / sqrt(x) if x > 0 else 0; bent when c < bend_cos, the
+ *            smallest double c with acos(c) 180 / pi <= 70 (found on the host against libm).
+ *   codes    DSSP 2.2.0's helix flags (strides 3, 4, 5), bridges (i, j >= i + 3) with its grouping and ladder merge in
+ *            its order, uint32 differences included, then E / B, H, G, I (no pi-helix priority), T and S.
+ *            codes[k * ld + r] uint8: 0 loop, 1 H, 2 B, 3 E, 4 G, 5 I, 6 T, 7 S; ld >= n_res.
+ * hb_partner [item][n_res][2] int32 and hb_energy [item][n_res][2] float64 (both NULL, or both given) receive both
+ * slots of every donor.  Per-frame state lives in global scratch (no residue limit in shared memory); the listed frames
+ * are processed in chunks of mkb_dssp_chunk_frames(n_res) items, so scratch stays bounded.  The handle's timing events
+ * bracket the whole call (main; prep is empty). */
+int mkb_dssp(mkb_handle_t h, void *stream, const mkb_traj *t, const int32_t *backbone, const uint8_t *flags,
+             int64_t n_res, double bend_cos, const uint32_t *frames, int64_t n_frames, uint8_t *codes, int64_t ld,
+             int32_t *hb_partner, double *hb_energy);
+int64_t mkb_dssp_chunk_frames(int64_t n_res);
+
 #ifdef __cplusplus
 }
 #endif

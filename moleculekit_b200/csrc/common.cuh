@@ -44,6 +44,7 @@ enum ScratchSlot {
     S_SASA_START,   // K17: first sorted record of every bucket
     S_SASA_MAXR,    // K17: largest radius
     S_SASA_AREA,    // K17: per-atom areas before the group sums
+    S_DSSP,         // K18: the per-frame arrays of one frame chunk, carved from one allocation
     S_NSLOTS
 };
 

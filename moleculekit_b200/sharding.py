@@ -157,6 +157,11 @@ def project_sharded(projection, mol, *, gather: bool = True, group=None):
         raise ValueError("project_sharded would take each rank's mean over its own frames: a MetricFluctuation without "
                          "refmol deviates from the mean over all frames, use sharding.fluctuation_sharded")
     world, rank = world_info(group)
+    from .projections.metricsecondarystructure import MetricSecondaryStructure
+
+    if gather and world > 1 and isinstance(projection, MetricSecondaryStructure) and not projection._integer:
+        raise ValueError("project_sharded cannot all_gather string rows: use MetricSecondaryStructure(integer=True), "
+                         "or gather=False")
     F = mol.numFrames
     off = partition(F, world)
     f0, f1 = int(off[rank]), int(off[rank + 1])
