@@ -82,7 +82,7 @@ struct mkb_ctx {
     // side stream of the occupancy run path (gate-band pre-pass beside the list build)
     cudaStream_t aux_stream = nullptr, aux_stream2 = nullptr;
     bool index_pending = false;  // mkb_occupancy_grid_batch_to_host: the block index is on its way to the host (aux_ev[3])
-    cudaEvent_t aux_ev[2 + 16] = {};  // band fork / join, one per chunk of the list-build pipeline
+    cudaEvent_t aux_ev[4] = {};  // band fork / join; block-index copy of the to-host route (issued / done)
     // K4: the count call leaves one ballot word per (row, 32 columns); the fill call that follows with the SAME arguments
     // reads them instead of evaluating every distance a second time
     struct K4Key {

@@ -5,8 +5,8 @@
 // flush, FFMA.SAT gate ...) are in the git history of this file together with their compile-time selectors.
 //
 //   * K2' (occ_prep_kernel / occ_blk_fill_kernel): every atom is appended to the candidate list of each 4x4x8-voxel
-//     block it can reach (~16 blocks per atom at 1 A) -- count, scan, fill.  The fill kernel reads its list; no block
-//     scans cell rows.
+//     block it can reach (~16 blocks per atom at 1 A) -- count, scan, fill, both walks counting per CTA and block in
+//     shared memory.  The fill kernel reads its list; no block scans cell rows.
 //   * value = max_a [d2 < cut2] f(sigma^2 / d2) with f monotone: the kernel tracks  r = d2 / sigma^2  as a MIN and applies f
 //     once per voxel-channel; no reciprocal per pair.
 //   * One warp owns a block; a lane owns the 4 voxels of one x-row (they share dy, dz).  The candidate is WARP-UNIFORM (two
@@ -67,7 +67,6 @@ struct RunParams {
     const double *sigmas;        // multi-sigma atoms only
     float *out;
     const long long *item_base;  // [B + 1]: first queue item of every grid (item = 4 x 4 voxels in x, y and R_ZC blocks in z)
-    unsigned item0;              // first item of this launch's chunk of grids (queue ids are chunk-local)
     int zc;                      // z blocks per item: R_ZC, or fewer when the batch has too few items to balance the resident warps
     unsigned *queue;
     unsigned total_items;
@@ -110,15 +109,56 @@ __device__ __forceinline__ void for_each_block_in_reach(const GridDev &g, float 
     }
 }
 
+// The atoms of one CTA share most of their blocks (C3: ~4 200 insertions into ~700 blocks per 256 atoms), so both list
+// passes count per (CTA, block) in a shared-memory hash table keyed by the global block slot (tile_base + block id; a CTA
+// may span several grids; linear probing) and touch global memory once per occupied entry.  An insertion whose key finds
+// neither itself nor a free slot within L_PROBES slots goes to global memory directly.  Keys are never removed, so every
+// insertion of a key within a CTA takes the same route in both walks of the fill pass.  At fine voxel sizes the atoms
+// of a CTA reach far more blocks than the table holds (C5, 0.5 A: ~100 blocks per atom, ~9 000 per CTA); there the
+// host turns the table off (`table` = 0) and every insertion takes the direct route.
+constexpr int L_THREADS = 256;          // atoms per CTA of the two list passes
+constexpr int L_TABLE = 2048;           // hash slots per CTA (power of two)
+constexpr int L_PROBES = 8;             // linear-probing limit
+constexpr int L_STAGE = 4096;           // entries per CTA staged in shared memory by the fill pass
+constexpr int L_TABLE_MAX_REACH = 64;   // the host uses the table when an atom reaches at most this many blocks
+constexpr unsigned L_EMPTY = 0xffffffffu;
+constexpr int L_SLOTS = L_TABLE / L_THREADS;  // slots per thread in the fill pass's scan
+static_assert(L_TABLE <= 2048 && L_THREADS <= 256, "a staged entry packs slot (11 bits) | thread (8) | mask (9)");
+
+__device__ __forceinline__ unsigned list_hash(unsigned key) { return (key * 2654435761u) >> (32 - 11); }
+static_assert(L_TABLE == 1 << 11, "list_hash yields 11 bits");
+
+// slot of `key` in the table, inserting it when absent; -1: not in the table (no free slot within the probing limit)
+__device__ __forceinline__ int list_slot_insert(unsigned *s_key, unsigned key) {
+    unsigned h = list_hash(key);
+    for (int p = 0; p < L_PROBES; ++p, h = (h + 1) & (L_TABLE - 1)) {
+        unsigned k = s_key[h];
+        if (k == L_EMPTY) k = atomicCAS(s_key + h, L_EMPTY, key);
+        if (k == L_EMPTY || k == key) return (int)h;
+    }
+    return -1;
+}
+// slot of `key` in a table no thread inserts into any more; -1: absent
+__device__ __forceinline__ int list_slot_find(const unsigned *s_key, unsigned key) {
+    unsigned h = list_hash(key);
+    for (int p = 0; p < L_PROBES; ++p, h = (h + 1) & (L_TABLE - 1)) {
+        const unsigned k = s_key[h];
+        if (k == key) return (int)h;
+        if (k == L_EMPTY) return -1;
+    }
+    return -1;
+}
+__device__ __forceinline__ void list_table_clear(unsigned *s_key, unsigned *s_cnt) {
+    for (int i = threadIdx.x; i < L_TABLE; i += L_THREADS) { s_key[i] = L_EMPTY; s_cnt[i] = 0u; }
+}
+
 // per atom item: record + block counts.  sigma handling as occ_scatter_kernel (one sigma + channel mask; several
 // distinct sigmas -> multi flag and the per-channel path of the fill kernel).
-__global__ void __launch_bounds__(128) occ_prep_kernel(const float *__restrict__ coords, const double *__restrict__ sigmas,
-                                                       const double *__restrict__ radii, const unsigned *__restrict__ chanmask,
-                                                       const GridDev *__restrict__ grids, int B, long long it0, long long n_items,
-                                                       float4 *__restrict__ rec_pos, uint4 *__restrict__ rec_tag,
-                                                       unsigned *__restrict__ blk_count) {
-    const long long it = it0 + blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    if (it >= it0 + n_items) return;
+__device__ __forceinline__ void occ_prep_item(const float *__restrict__ coords, const double *__restrict__ sigmas,
+                                              const double *__restrict__ radii, const unsigned *__restrict__ chanmask,
+                                              const GridDev *__restrict__ grids, int B, long long it, float4 *__restrict__ rec_pos,
+                                              uint4 *__restrict__ rec_tag, unsigned *__restrict__ blk_count, int table,
+                                              unsigned *s_key, unsigned *s_cnt) {
     const int b = find_grid_item(grids, B, it);
     const GridDev &g = grids[b];
     const long long a = g.atom_begin + (it - g.item_base);
@@ -159,31 +199,117 @@ __global__ void __launch_bounds__(128) occ_prep_kernel(const float *__restrict__
     rec_tag[it] = make_uint4(live ? (m | (multi ? 0x100u : 0u) | ((unsigned)(ip[2] + off) << 16)) : 0u, (unsigned)a,
                              live ? ((unsigned)(ip[0] + off) | ((unsigned)(ip[1] + off) << 16)) : 0u, __float_as_uint(sw));
     if (!live) return;
-    unsigned *const bc = blk_count + g.tile_base;  // tile_base: first block of this grid
-    for_each_block_in_reach(g, (float)ip[0] + f[0], (float)ip[1] + f[1], (float)ip[2] + f[2], [&](int bid) { atomicAdd(bc + bid, 1u); });
+    const unsigned tb = (unsigned)g.tile_base;  // first block slot of this grid
+    for_each_block_in_reach(g, (float)ip[0] + f[0], (float)ip[1] + f[1], (float)ip[2] + f[2], [&](int bid) {
+        const int s = table ? list_slot_insert(s_key, tb + bid) : -1;
+        if (s >= 0) atomicAdd(s_cnt + s, 1u);
+        else atomicAdd(blk_count + tb + bid, 1u);
+    });
 }
 
-// second pass: the same walk appends (item, mask | multi << 8) to the lists; blk_count counts down to zero.  (Keeping the
-// slots of the first pass instead -- no atomics here -- was slower.)
-__global__ void __launch_bounds__(128) occ_blk_fill_kernel(const GridDev *__restrict__ grids, int B, long long it0, long long n_items,
-                                                           const float4 *__restrict__ rec_pos, const uint4 *__restrict__ rec_tag,
-                                                           unsigned *__restrict__ blk_count, const unsigned *__restrict__ blk_start,
-                                                           uint2 *__restrict__ blk_ent) {
-    const long long it = it0 + blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    if (it >= it0 + n_items) return;
-    const uint4 tg = rec_tag[it];
-    if ((tg.x & 0x1ffu) == 0) return;
-    const int b = find_grid_item(grids, B, it);
-    const GridDev &g = grids[b];
-    const float4 f = rec_pos[it];
-    const int off = g.cutv + 1;
-    const float px = (float)((int)(tg.z & 0xffffu) - off) + f.x, py = (float)((int)(tg.z >> 16) - off) + f.y,
-                pz = (float)((int)(tg.x >> 16) - off) + f.z;
-    unsigned *const bc = blk_count + g.tile_base;
-    const unsigned *const bs = blk_start + g.tile_base;
-    const uint2 ent = make_uint2((unsigned)it, tg.x & 0x1ffu);
-    uint2 *const be = blk_ent + g.ent_base;
-    for_each_block_in_reach(g, px, py, pz, [&](int bid) { be[bs[bid] + atomicSub(bc + bid, 1u) - 1u] = ent; });
+__global__ void __launch_bounds__(L_THREADS) occ_prep_kernel(const float *__restrict__ coords, const double *__restrict__ sigmas,
+                                                             const double *__restrict__ radii, const unsigned *__restrict__ chanmask,
+                                                             const GridDev *__restrict__ grids, int B, long long n_items,
+                                                             float4 *__restrict__ rec_pos, uint4 *__restrict__ rec_tag,
+                                                             unsigned *__restrict__ blk_count, int table) {
+    __shared__ unsigned s_key[L_TABLE], s_cnt[L_TABLE];
+    list_table_clear(s_key, s_cnt);
+    __syncthreads();
+    const long long it = blockIdx.x * (long long)L_THREADS + threadIdx.x;
+    if (it < n_items) occ_prep_item(coords, sigmas, radii, chanmask, grids, B, it, rec_pos, rec_tag, blk_count, table, s_key, s_cnt);
+    __syncthreads();
+    for (int i = threadIdx.x; i < L_TABLE; i += L_THREADS)
+        if (s_key[i] != L_EMPTY) atomicAdd(blk_count + s_key[i], s_cnt[i]);
+}
+
+// second pass: the same walk appends (item, mask | multi << 8) to the lists; blk_count counts down to zero.  Walk 1 counts
+// the CTA's insertions per block in the table, one atomicSub per occupied entry reserves the segment [old - n, old) of
+// that block's list, and walk 2 places every insertion at its segment's base + a shared cursor.  The first L_STAGE
+// entries of the CTA are staged in shared memory in segment order (one word: table slot, thread, mask) and leave in one
+// pass at the end, consecutive threads writing consecutive list positions (one scattered 8-byte store per entry took
+// most of the pass); entries beyond L_STAGE are stored at once.  Insertions outside the table reserve and store their
+// entry one by one.  (Keeping the slots of the first pass instead was slower.)
+__global__ void __launch_bounds__(L_THREADS, 5) occ_blk_fill_kernel(const GridDev *__restrict__ grids, int B, long long n_items,
+                                                                 const float4 *__restrict__ rec_pos, const uint4 *__restrict__ rec_tag,
+                                                                 unsigned *__restrict__ blk_count, const unsigned *__restrict__ blk_start,
+                                                                 uint2 *__restrict__ blk_ent, int table) {
+    // keys, cursors, list position - staged index per slot; staged entries; warp sums of the scan
+    __shared__ unsigned s_key[L_TABLE], s_cur[L_TABLE], s_off[L_TABLE], s_stage[L_STAGE], s_wsum[L_THREADS / 32];
+    list_table_clear(s_key, s_cur);
+    __syncthreads();
+    const long long it = blockIdx.x * (long long)L_THREADS + threadIdx.x;
+    uint4 tg = make_uint4(0u, 0u, 0u, 0u);
+    if (it < n_items) tg = rec_tag[it];
+    const bool live = (tg.x & 0x1ffu) != 0;
+    const GridDev *g = nullptr;
+    float px = 0.0f, py = 0.0f, pz = 0.0f;
+    if (live) {
+        g = grids + find_grid_item(grids, B, it);
+        const float4 f = rec_pos[it];
+        const int off = g->cutv + 1;
+        px = (float)((int)(tg.z & 0xffffu) - off) + f.x;
+        py = (float)((int)(tg.z >> 16) - off) + f.y;
+        pz = (float)((int)(tg.x >> 16) - off) + f.z;
+        const unsigned tb = (unsigned)g->tile_base;
+        if (table)  // without the table walk 2 finds every key absent
+            for_each_block_in_reach(*g, px, py, pz, [&](int bid) {
+                const int s = list_slot_insert(s_key, tb + bid);
+                if (s >= 0) atomicAdd(s_cur + s, 1u);
+            });
+    }
+    __syncthreads();
+    // segments in slot order: thread t scans L_SLOTS consecutive slots, the staged order is an exclusive scan of the counts
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned n[L_SLOTS], sum = 0;
+#pragma unroll
+    for (int j = 0; j < L_SLOTS; ++j) { n[j] = s_cur[threadIdx.x * L_SLOTS + j]; sum += n[j]; }
+    unsigned incl = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+    }
+    if (lane == 31) s_wsum[warp] = incl;
+    __syncthreads();
+    unsigned loff = incl - sum, total = 0;
+#pragma unroll
+    for (int w = 0; w < L_THREADS / 32; ++w) {
+        const unsigned ws = s_wsum[w];
+        loff += w < warp ? ws : 0u;
+        total += ws;
+    }
+#pragma unroll
+    for (int j = 0; j < L_SLOTS; ++j) {
+        const int i = threadIdx.x * L_SLOTS + j;
+        const unsigned key = s_key[i];
+        if (key != L_EMPTY) {
+            s_off[i] = blk_start[key] + atomicSub(blk_count + key, n[j]) - n[j] - loff;  // list position - staged index
+            s_cur[i] = loff;
+        }
+        loff += n[j];
+    }
+    __syncthreads();
+    if (live) {
+        const unsigned tb = (unsigned)g->tile_base;
+        const uint2 ent = make_uint2((unsigned)it, tg.x & 0x1ffu);
+        for_each_block_in_reach(*g, px, py, pz, [&](int bid) {
+            const unsigned key = tb + bid;
+            const int s = list_slot_find(s_key, key);
+            if (s >= 0) {
+                const unsigned li = atomicAdd(s_cur + s, 1u);
+                if (li < (unsigned)L_STAGE) s_stage[li] = (unsigned)s << 17 | threadIdx.x << 9 | ent.y;
+                else blk_ent[s_off[s] + li] = ent;
+            } else {
+                blk_ent[blk_start[key] + atomicSub(blk_count + key, 1u) - 1u] = ent;
+            }
+        });
+    }
+    __syncthreads();
+    const unsigned it0 = (unsigned)(blockIdx.x * L_THREADS);
+    for (unsigned i = threadIdx.x; i < min(total, (unsigned)L_STAGE); i += L_THREADS) {
+        const unsigned w = s_stage[i];
+        blk_ent[s_off[w >> 17] + i] = make_uint2(it0 + ((w >> 9) & 0xffu), w & 0x1ffu);
+    }
 }
 
 // compact output: 1 for every block with a candidate list, then an exclusive scan gives its record index
@@ -280,7 +406,7 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
             gi = (int)(id / p.u_ipg);
             local = id - (unsigned)gi * p.u_ipg;
         } else {
-            const long long gid = (long long)id + p.item0;
+            const long long gid = (long long)id;
             int lo = 0, hi = p.B - 1;
             while (lo < hi) {
                 const int mid = (lo + hi + 1) >> 1;
@@ -729,7 +855,7 @@ __device__ __forceinline__ void occ_fix_voxel(const GridDev *__restrict__ grids,
 #pragma unroll
     for (int h = 0; h < 8; ++h) q[h] = 0.0;
     for (unsigned i = e0 + lane; i < e1; i += 32) {
-        const unsigned a = __ldg(&rec_tag[__ldg(&blk_ent[g->ent_base + i].x)].y);
+        const unsigned a = __ldg(&rec_tag[__ldg(&blk_ent[i].x)].y);
         const double dx = (double)coords[3ll * a + 0] - cx;
         const double dy = (double)coords[3ll * a + 1] - cy;
         const double dz = (double)coords[3ll * a + 2] - cz;

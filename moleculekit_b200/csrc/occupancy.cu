@@ -53,7 +53,6 @@ struct GridDev {
     long long atom_begin, atom_end, out_offset;
     long long item_base, tile_base, cell_base;
     long long vox_base;  // first voxel of this grid in the dense batch order (gate-band bitmap of the run kernel)
-    long long ent_base;  // run kernel: where the candidate lists of this grid's chunk start in blk_ent
 };
 
 __device__ __forceinline__ float rcp_approx(float x) {
@@ -1667,14 +1666,9 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
     // tests/test_occupancy_gpu.py::test_alternative_kernel_paths_agree); accumulate calls stay on v6 as well.
     bool use_runs = (variant == 0 || (variant == 1 && !getenv("MKB_OCC_TILE"))) && C == 8 && !(flags & MKB_OCC_ACCUMULATE) && ((uintptr_t)out % 16 == 0) &&
                     !getenv("MKB_OCC_V6") && !force_warp && !getenv("MKB_OCC_WARP32");
-    // The batch can be cut into chunks of grids (MKB_OCC_CHUNKS=n): the list build of chunk c + 1 then runs on a side stream
-    // beside the fill kernel of chunk c.  Chunk c owns the slots [blk_off[c], blk_off[c + 1]) of blk_count / blk_start (its
-    // blocks + 1: every chunk has its own exclusive scan) and the entries from ent_off[c] on.  The list build does not
-    // hide behind the persistent fill kernel and every extra launch adds a tail, so the default is ONE chunk.
-    int n_chunks = 1;
-    std::vector<int> cgrid;                // [n_chunks + 1] first grid of every chunk
-    std::vector<long long> blk_off, ent_off, item_off, atom_item_off, ibase;
+    std::vector<long long> ibase;
     long long run_blocks = 0, run_items = 0, ent_bound = 0;
+    int list_table = 1;  // the list passes count per CTA in shared memory (occ_runs.cuh): off for fine voxels
     int run_zc = R_ZC;
     if (use_runs) {
         std::vector<long long> nblk((size_t)B), nitem((size_t)B), nent((size_t)B);
@@ -1699,38 +1693,18 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
             const long long rx = std::min<long long>(nbx, (long long)((c2 + 3) / 4) + 1), ry = std::min<long long>(nby, (long long)((c2 + 3) / 4) + 1),
                             rz = std::min<long long>(nbz, (long long)((c2 + R_BZ - 1) / R_BZ) + 1);
             nent[b] = (g.atom_end - g.atom_begin) * rx * ry * rz;
+            if (rx * ry * rz > L_TABLE_MAX_REACH) list_table = 0;
             run_blocks += nblk[b]; run_items += nitem[b]; ent_bound += nent[b];
         }
         if (run_blocks >= (1ll << 31) - 64 || ent_bound >= (1ll << 32) - 1) use_runs = false;
         if (use_runs) {
-            const char *ce = getenv("MKB_OCC_CHUNKS");
-            n_chunks = blk_rank ? 1 : (ce ? std::max(1, atoi(ce)) : 1);  // compact output numbers its records with one scan
-            n_chunks = std::max(1, std::min(std::min(n_chunks, 16), B / 8));
-            cgrid.assign((size_t)n_chunks + 1, B);
-            cgrid[0] = 0;
-            long long acc = 0;
-            for (int b = 0, c = 1; b < B && c < n_chunks; ++b) {  // cut where the running block count crosses c / n_chunks
-                acc += nblk[b];
-                if (acc * n_chunks >= run_blocks * c) cgrid[c++] = b + 1;
-            }
-            for (int c = 1; c <= n_chunks; ++c) cgrid[c] = std::max(cgrid[c], cgrid[c - 1]);
-            blk_off.assign((size_t)n_chunks + 1, 0); ent_off.assign((size_t)n_chunks + 1, 0);
-            item_off.assign((size_t)n_chunks + 1, 0); atom_item_off.assign((size_t)n_chunks + 1, 0);
             ibase.assign((size_t)B + 1, 0);
-            for (int c = 0; c < n_chunks; ++c) {
-                long long bsum = 0, esum = 0, isum = 0, asum = 0;
-                for (int b = cgrid[c]; b < cgrid[c + 1]; ++b) {
-                    gd[b].tile_base = blk_off[c] + bsum;  // first 4x4x8 block of this grid (slot index)
-                    gd[b].ent_base = ent_off[c];
-                    ibase[b] = item_off[c] + isum;
-                    bsum += nblk[b]; esum += nent[b]; isum += nitem[b]; asum += gd[b].atom_end - gd[b].atom_begin;
-                }
-                blk_off[c + 1] = blk_off[c] + bsum + 1;  // + 1: the chunk's total after its exclusive scan
-                ent_off[c + 1] = ent_off[c] + esum;
-                item_off[c + 1] = item_off[c] + isum;
-                atom_item_off[c + 1] = atom_item_off[c] + asum;
+            long long bsum = 0;
+            for (int b = 0; b < B; ++b) {
+                gd[b].tile_base = bsum;  // first 4x4x8 block of this grid (slot index)
+                bsum += nblk[b];
+                ibase[b + 1] = ibase[b] + nitem[b];
             }
-            ibase[B] = run_items;
         }
     }
     if (blk_rank && !use_runs)
@@ -1750,7 +1724,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         const size_t ni = (size_t)std::max<long long>(items, 1);
         const long long n_words = cdiv(voxels, 32);
         const unsigned fix_cap = (unsigned)std::min<long long>(voxels, 1ll << 22);
-        const size_t nslots = (size_t)blk_off[n_chunks];
+        const size_t nslots = (size_t)run_blocks + 1;  // + 1: the total after the exclusive scan
         if ((rc = scratch_get(h, S_DESC, (size_t)B, &d_grids))) return rc;
         if ((rc = scratch_get(h, S_SORT_PX, ni, &rec_pos))) return rc;
         if ((rc = scratch_get(h, S_SORT_PY, ni, &rec_tag))) return rc;
@@ -1761,14 +1735,11 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         if ((rc = scratch_get(h, S_BAND_BITMAP, (size_t)n_words, &d_bitmap))) return rc;
         if ((rc = scratch_get(h, S_QUEUE, (size_t)64, &d_queue))) return rc;
         if ((rc = scratch_get(h, S_FIX_LIST, (size_t)fix_cap + FIX_HDR, &d_fix))) return rc;
-        // cub temp storage for the scans, sized before anything is enqueued (the scans run on the side stream)
+        // cub temp storage for the scans, sized before anything is enqueued
         unsigned *scan_tmp = nullptr;
         size_t scan_bytes = 0;
         {
-            long long mx = 0;
-            for (int c = 0; c < n_chunks; ++c) mx = std::max(mx, blk_off[c + 1] - blk_off[c]);
-            mx = std::max(mx, run_blocks + 1);
-            MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, blk_count, blk_start, (int)mx, st));
+            MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, blk_count, blk_start, (int)nslots, st));
             void *tmp = nullptr;
             if ((rc = scratch_get(h, S_SCAN_TMP, scan_bytes, &tmp))) return rc;
             scan_tmp = static_cast<unsigned *>(tmp);
@@ -1794,88 +1765,81 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         MKB_CUDA(h, cudaMemsetAsync(d_bitmap, 0, sizeof(unsigned) * (size_t)n_words, st));
         MKB_CUDA(h, cudaMemsetAsync(d_queue, 0, sizeof(unsigned) * 64, st));
         MKB_CUDA(h, cudaMemsetAsync(d_fix, 0, sizeof(unsigned long long) * FIX_HDR, st));
-        cudaStream_t sk = n_chunks > 1 ? h->aux_stream2 : st;  // list builds
         // the gate-band pre-pass (compute bound) runs beside the list build (atomic bound) on a side stream; small calls
         // keep it on the caller's stream (the fork / join costs more host time than the overlap saves)
         const bool band_aside = items >= 200000;
         if (items > 0) {
-            if (band_aside || sk != st) MKB_CUDA(h, cudaEventRecord(h->aux_ev[0], st));
             cudaStream_t sb = band_aside ? h->aux_stream : st;
-            if (band_aside) MKB_CUDA(h, cudaStreamWaitEvent(sb, h->aux_ev[0], 0));
+            if (band_aside) {
+                MKB_CUDA(h, cudaEventRecord(h->aux_ev[0], st));
+                MKB_CUDA(h, cudaStreamWaitEvent(sb, h->aux_ev[0], 0));
+            }
             occ_band_kernel<<<(unsigned)cdiv(items, 128), 128, 0, sb>>>(coords, d_grids, B, items, d_bitmap, d_fix, fix_cap);
             MKB_LAUNCHED(h);
             if (band_aside) MKB_CUDA(h, cudaEventRecord(h->aux_ev[1], sb));
-            if (sk != st) MKB_CUDA(h, cudaStreamWaitEvent(sk, h->aux_ev[0], 0));
         }
         h->last_kernel = "occ_fill_runs_kernel";
-        for (int c = 0; c < n_chunks; ++c) {
-            const int g0 = cgrid[c], g1 = cgrid[c + 1];
-            if (g1 == g0) continue;
-            const long long it0 = atom_item_off[c], nit = atom_item_off[c + 1] - it0;
-            const long long nb1 = blk_off[c + 1] - blk_off[c];  // blocks + 1
-            if (nit > 0) {
-                occ_prep_kernel<<<(unsigned)cdiv(nit, 128), 128, 0, sk>>>(coords, sigmas, radii, chanmask, d_grids, B, it0, nit, rec_pos, rec_tag, blk_count);
-                MKB_LAUNCHED(h);
-            }
-            MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, blk_count + blk_off[c], blk_start + blk_off[c], (int)nb1, sk));
+        if (items > 0) {
+            occ_prep_kernel<<<(unsigned)cdiv(items, L_THREADS), L_THREADS, 0, st>>>(coords, sigmas, radii, chanmask, d_grids, B, items, rec_pos, rec_tag, blk_count, list_table);
+            MKB_LAUNCHED(h);
+        }
+        MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, blk_count, blk_start, (int)nslots, st));
+        h->launches++;
+        if (items > 0) {
+            occ_blk_fill_kernel<<<(unsigned)cdiv(items, L_THREADS), L_THREADS, 0, st>>>(d_grids, B, items, rec_pos, rec_tag, blk_count, blk_start, blk_ent, list_table);
+            MKB_LAUNCHED(h);
+        }
+        if (blk_rank) {  // record index of every non-empty block (blk_count is free again after the list fill)
+            occ_blk_flag_kernel<<<(unsigned)cdiv(run_blocks + 1, 256), 256, 0, st>>>(blk_start, run_blocks, blk_count);
+            MKB_LAUNCHED(h);
+            MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, blk_count, blk_rank, (int)(run_blocks + 1), st));
             h->launches++;
-            if (nit > 0) {
-                occ_blk_fill_kernel<<<(unsigned)cdiv(nit, 128), 128, 0, sk>>>(d_grids, B, it0, nit, rec_pos, rec_tag, blk_count, blk_start, blk_ent);
-                MKB_LAUNCHED(h);
+            if (host_rank) {  // the block index leaves for the host NOW (side stream), before the fill kernel starts
+                MKB_CUDA(h, cudaEventRecord(h->aux_ev[2], st));
+                MKB_CUDA(h, cudaStreamWaitEvent(h->aux_stream2, h->aux_ev[2], 0));
+                MKB_CUDA(h, cudaMemcpyAsync(host_rank, blk_rank, sizeof(uint32_t) * (size_t)(run_blocks + 1), cudaMemcpyDeviceToHost, h->aux_stream2));
+                MKB_CUDA(h, cudaEventRecord(h->aux_ev[3], h->aux_stream2));
+                h->index_pending = true;
             }
-            if (blk_rank) {  // record index of every non-empty block (blk_count is free again after the list fill); one chunk
-                occ_blk_flag_kernel<<<(unsigned)cdiv(run_blocks + 1, 256), 256, 0, sk>>>(blk_start, run_blocks, blk_count);
-                MKB_LAUNCHED(h);
-                MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, blk_count, blk_rank, (int)(run_blocks + 1), sk));
-                h->launches++;
-                if (host_rank) {  // the block index leaves for the host NOW (side stream), before the fill kernel starts
-                    MKB_CUDA(h, cudaEventRecord(h->aux_ev[2], sk));
-                    MKB_CUDA(h, cudaStreamWaitEvent(h->aux_stream2, h->aux_ev[2], 0));
-                    MKB_CUDA(h, cudaMemcpyAsync(host_rank, blk_rank, sizeof(uint32_t) * (size_t)(run_blocks + 1), cudaMemcpyDeviceToHost, h->aux_stream2));
-                    MKB_CUDA(h, cudaEventRecord(h->aux_ev[3], h->aux_stream2));
-                    h->index_pending = true;
-                }
-            }
-            if (sk != st) {
-                MKB_CUDA(h, cudaEventRecord(h->aux_ev[2 + c], sk));
-                MKB_CUDA(h, cudaStreamWaitEvent(st, h->aux_ev[2 + c], 0));
-            }
+        }
+        {
             RunParams rp;
-            rp.grids = d_grids + g0; rp.B = g1 - g0;
-            rp.rec_pos = rec_pos; rp.rec_tag = rec_tag; rp.blk_start = blk_start; rp.blk_ent = blk_ent + ent_off[c];
+            rp.grids = d_grids; rp.B = B;
+            rp.rec_pos = rec_pos; rp.rec_tag = rec_tag; rp.blk_start = blk_start; rp.blk_ent = blk_ent;
             rp.sigmas = sigmas; rp.out = out;
-            rp.item_base = d_ibase + g0; rp.item0 = (unsigned)item_off[c]; rp.queue = d_queue + c;
-            rp.total_items = (unsigned)(item_off[c + 1] - item_off[c]);
+            rp.item_base = d_ibase; rp.queue = d_queue;
+            rp.total_items = (unsigned)run_items;
             rp.cmajor = (flags & MKB_OCC_LAYOUT_CXYZ) ? 1 : 0;
             rp.blk_rank = blk_rank;
             rp.sparse_dense = host_rank ? 1 : 0;
             bool uni = true;
-            const GridDev &g0d = gd[g0];
+            const GridDev &g0d = gd[0];
             const long long nvox0 = (long long)g0d.dims[0] * g0d.dims[1] * g0d.dims[2];
-            for (int b = g0; b < g1 && uni; ++b) {
+            for (int b = 0; b < B && uni; ++b) {
                 const GridDev &g = gd[b];
                 uni = g.dims[0] == g0d.dims[0] && g.dims[1] == g0d.dims[1] && g.dims[2] == g0d.dims[2] && g.vs == g0d.vs &&
-                      g.out_offset == g0d.out_offset + (b - g0) * nvox0;
+                      g.out_offset == g0d.out_offset + b * nvox0;
             }
             rp.u = g0d;
             rp.u_out_stride = nvox0;
-            rp.u_ipg = (unsigned)(ibase[g0 + 1] - ibase[g0]);
+            rp.u_ipg = (unsigned)(ibase[1] - ibase[0]);
             rp.u_nby = (unsigned)((g0d.dims[1] + 3) / 4);
             rp.u_nzc = (unsigned)(((g0d.dims[2] + R_BZ - 1) / R_BZ + run_zc - 1) / run_zc);
             rp.zc = run_zc;
-            rp.u_bpg = (unsigned)(g1 - g0 > 1 ? gd[g0 + 1].tile_base - g0d.tile_base : 0);
-            if (h->timing && c == 0) MKB_CUDA(h, cudaEventRecord(h->ev[1], st));
+            rp.u_bpg = (unsigned)(B > 1 ? gd[1].tile_base - g0d.tile_base : 0);
+            if (h->timing) MKB_CUDA(h, cudaEventRecord(h->ev[1], st));
             const unsigned nctas = (unsigned)std::min<long long>((long long)h->sm_count * MKB_R_MIN_CTAS, cdiv((long long)rp.total_items, R_WARPS));
-            if (nctas == 0) continue;
             rp.use_tmap = 0;
             CUtensorMap tmap;
             memset(&tmap, 0, sizeof(tmap));
             // dense uniform output in device memory (the to-host route writes mapped host memory: row copies)
             if (uni && !rp.cmajor && !rp.blk_rank && !getenv("MKB_OCC_NO_TMAP"))
-                rp.use_tmap = occ_make_tmap(&tmap, out + g0d.out_offset * 8, g0d.dims[0], g0d.dims[1], g0d.dims[2], g1 - g0, nvox0) ? 1 : 0;
-            if (uni) occ_fill_runs_kernel<true><<<nctas, R_WARPS * 32, 0, st>>>(rp, tmap);
-            else occ_fill_runs_kernel<false><<<nctas, R_WARPS * 32, 0, st>>>(rp, tmap);
-            MKB_LAUNCHED(h);
+                rp.use_tmap = occ_make_tmap(&tmap, out + g0d.out_offset * 8, g0d.dims[0], g0d.dims[1], g0d.dims[2], B, nvox0) ? 1 : 0;
+            if (nctas > 0) {
+                if (uni) occ_fill_runs_kernel<true><<<nctas, R_WARPS * 32, 0, st>>>(rp, tmap);
+                else occ_fill_runs_kernel<false><<<nctas, R_WARPS * 32, 0, st>>>(rp, tmap);
+                MKB_LAUNCHED(h);
+            }
         }
         if (h->timing) MKB_CUDA(h, cudaEventRecord(h->ev[2], st));
         if (items > 0) {
