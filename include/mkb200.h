@@ -472,6 +472,38 @@ int mkb_dssp(mkb_handle_t h, void *stream, const mkb_traj *t, const int32_t *bac
              int32_t *hb_partner, double *hb_energy);
 int64_t mkb_dssp_chunk_frames(int64_t n_res);
 
+/* K19: TM-score, replaces the superposition search of the TMscore program (Zhang & Skolnick, Proteins 2004) that
+ * moleculekit's molTMscore runs per frame.  All pointers except the mkb_traj structs, frag and the scalars are device
+ * pointers.  Pair k (0 <= k < L = n_pairs, 1 <= L <= mkb_tmscore_max_pairs()) joins atom row sel[k] of t (model x_k) and
+ * atom row refsel[k] of frame 0 of ref (reference y_k).  l_norm >= 1 is the normaliser.  d0 > 0, d0_search and frag
+ * [n_frag] host int32 (1 <= n_frag <= 6, each in [1, L]) are computed by the caller: d0 = 0.5 if l_norm <= 15, else
+ * max(0.5, 1.24 pow(l_norm - 15, 1/3) - 1.8); d0_search = d0 clamped to [4.5, 8]; frag = floor(L / 2^i) for i = 0..4
+ * while it is > min(4, L), then min(4, L).  frames [n_frames] uint32 = the listed frames of t (NULL = every frame,
+ * n_frames ignored); item k is frame frames[k].  Index ranges are the caller's responsibility.
+ *
+ * Per item, everything in float64 from the float32 coordinates, every operation rounded on its own (no fused
+ * multiply-add), every sum sequential in ascending pair order:
+ *   fit      of a pair set of size c: p = (sum x) / c, q = (sum y) / c, H[a][b] = sum (x_a - p_a)(y_b - q_b) in a second
+ *            pass; R = the rotation of Horn's quaternion (the eigenvector of the largest eigenvalue of the symmetric 4x4
+ *            matrix by cyclic Jacobi, at most 50 sweeps, the "late" threshold after sweep 3, ties to the lowest index);
+ *            x' = R (x - p) + q, each row ((R0 a0 + R1 a1) + R2 a2) + q.
+ *   score    over all L pairs: dis = sqrt((dx dx + dy dy) + dz dz), d = x' - y, t = dis / d0; S = (sum 1 / (1 + t t)) /
+ *            l_norm.
+ *   cut      the pairs with dis < dcut; while fewer than 3 and L > 3, dcut (a local copy) grows by 0.5 and the pairs are
+ *            cut again, at most 2^20 times.
+ *   search   for every fragment length Li in order and every start iL = 0..L - Li: fit the pairs iL..iL + Li - 1 and
+ *            cut at d0_search - 1; then up to 20 times: stop if the cut set is empty, fit the cut set, cut at
+ *            d0_search + 1, stop if the new set equals the one just fitted.
+ *   output   tm[k] = the largest S of every fit of every seed; rmsd[k] = sqrt((sum |x' - y|^2) / L) under the first
+ *            fit (the all-pairs one).  A non-finite coordinate among the pairs gives NaN for both, in that item only.
+ * Two bitmasks of L bits per resident thread live in global scratch.  The handle's timing events bracket the kernel
+ * (main; prep is empty). */
+int mkb_tmscore(mkb_handle_t h, void *stream, const mkb_traj *t, const uint32_t *sel, const mkb_traj *ref,
+                const uint32_t *refsel, int64_t n_pairs, int64_t l_norm, double d0, double d0_search,
+                const int32_t *frag, int32_t n_frag, const uint32_t *frames, int64_t n_frames, double *tm,
+                double *rmsd);
+int64_t mkb_tmscore_max_pairs(void);
+
 #ifdef __cplusplus
 }
 #endif

@@ -43,6 +43,7 @@ EXPORTS = [
     "mkb_wrap_triclinic", "mkb_hbonds_count", "mkb_hbonds_fill", "mkb_ring_pairs_count", "mkb_ring_pairs_fill",
     "mkb_align_fit", "mkb_align_apply", "mkb_rmsd", "mkb_coordinates", "mkb_coord_sums", "mkb_fluctuation",
     "mkb_dihedrals", "mkb_sasa", "mkb_sasa_chunk_frames", "mkb_dssp", "mkb_dssp_chunk_frames",
+    "mkb_tmscore", "mkb_tmscore_max_pairs",
 ]
 
 _lib = None
@@ -126,9 +127,12 @@ def load():
     lib.mkb_dssp.argtypes = [vp, vp, tp, vp, vp, i64, C.c_double, vp, i64, vp, i64, vp, vp]
     lib.mkb_dssp_chunk_frames.argtypes = [i64]
     lib.mkb_dssp_chunk_frames.restype = i64
+    lib.mkb_tmscore.argtypes = [vp, vp, tp, vp, tp, vp, i64, i64, C.c_double, C.c_double, vp, i32, vp, i64, vp, vp]
+    lib.mkb_tmscore_max_pairs.argtypes = []
+    lib.mkb_tmscore_max_pairs.restype = i64
     for name in EXPORTS:
         if name in ("mkb_last_error", "mkb_launch_count", "mkb_version", "mkb_last_kernel", "mkb_occupancy_compact_blocks",
-                    "mkb_sasa_chunk_frames", "mkb_dssp_chunk_frames"):
+                    "mkb_sasa_chunk_frames", "mkb_dssp_chunk_frames", "mkb_tmscore_max_pairs"):
             continue
         getattr(lib, name).restype = C.c_int
     _lib = lib

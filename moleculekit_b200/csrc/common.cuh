@@ -45,6 +45,7 @@ enum ScratchSlot {
     S_SASA_MAXR,    // K17: largest radius
     S_SASA_AREA,    // K17: per-atom areas before the group sums
     S_DSSP,         // K18: the per-frame arrays of one frame chunk, carved from one allocation
+    S_TMSCORE_MASK, // K19: two cut-set bitmasks per resident thread
     S_NSLOTS
 };
 
