@@ -41,9 +41,11 @@ typedef enum {
 typedef struct mkb_ctx *mkb_handle_t;
 
 /* flags for the occupancy entry points */
-#define MKB_OCC_ACCUMULATE 1u /* out = max(out, value): the reference accumulates into the caller's buffer
-                                 (occupancy_utils.pyx:61); without it `out` is overwritten (caller passes zeros,
-                                 voxeldescriptors.py:531, so both agree) */
+#define MKB_OCC_ACCUMULATE 1u /* out = value if value > out, as the reference accumulates into the caller's buffer
+                                 (occupancy_utils.pyx:56-61): only voxel-channels that some atom with a non-zero sigma
+                                 reaches within 5 A are updated; the others keep their bits (a negative, -inf or NaN
+                                 prefill included), and NaN in `out` sticks.  Without it `out` is overwritten (caller
+                                 passes zeros, voxeldescriptors.py:531, so both agree) */
 #define MKB_OCC_LAYOUT_CXYZ 2u /* SURVEY 8f row 1: grid b is written channel-major, out[b] = float32 [C][nx][ny][nz]
                                  (the layout a Conv3d consumer wants, instead of the reference's [nx][ny][nz][C]
                                  reshaped view, voxeldescriptors.py:298-299); grid b still starts at out + out_offset*C.

@@ -444,7 +444,7 @@ __global__ void __launch_bounds__(FILL_THREADS, (CP <= 8 ? 2 : 1)) occ_fill_kern
         if (p.flags & MKB_OCC_ACCUMULATE) {
 #pragma unroll
             for (int h = 0; h < CP; ++h)
-                if (h < C) { const float old = o[h * cs]; v[h] = (v[h] > old) ? v[h] : old; }  // pyx:61 `value > old`
+                if (h < C) { const float old = o[h * cs]; v[h] = (acc[h] > 0.0f && v[h] > old) ? v[h] : old; }  // pyx:61 `value > old`
         }
         if (CP == 8 && p.vec_ok) {
             __stcs(reinterpret_cast<float4 *>(o), make_float4(v[0], v[1], v[2], v[3]));
@@ -780,7 +780,7 @@ __global__ void __launch_bounds__(FILL_THREADS, 2) occ_fill8_kernel(const FillPa
         if (p.flags & MKB_OCC_ACCUMULATE) {
 #pragma unroll
             for (int h = 0; h < 8; ++h)
-                if (h < C) { const float old = oo[h * cs]; v[h] = (v[h] > old) ? v[h] : old; }
+                if (h < C) { const float old = oo[h * cs]; v[h] = (acc[h] > 0.0f && v[h] > old) ? v[h] : old; }
         }
         if (p.vec_ok) {
             __stcs(reinterpret_cast<float4 *>(oo), make_float4(v[0], v[1], v[2], v[3]));
@@ -1070,7 +1070,7 @@ __global__ void __launch_bounds__(W_WARPS * 32, W_MIN_CTAS) occ_fill8w_kernel(co
         if (p.flags & MKB_OCC_ACCUMULATE) {
 #pragma unroll
             for (int h = 0; h < 8; ++h)
-                if (h < C) { const float old = oo[h * cs]; v[h] = (v[h] > old) ? v[h] : old; }
+                if (h < C) { const float old = oo[h * cs]; v[h] = (acc[h] > 0.0f && v[h] > old) ? v[h] : old; }
         }
         if (p.vec_ok) {
             __stcs(reinterpret_cast<float4 *>(oo), make_float4(v[0], v[1], v[2], v[3]));
@@ -1425,7 +1425,10 @@ occ_fill8v_kernel(const FillParams p, const long long *__restrict__ block_base, 
             if (p.flags & MKB_OCC_ACCUMULATE) {
 #pragma unroll
                 for (int h = 0; h < 8; ++h)
-                    if (h < C) { const float old = oo[h * cs]; val[h] = (val[h] > old) ? val[h] : old; }
+                    if (h < C) {
+                        const float old = oo[h * cs], q = v == 0 ? acc0[h] : acc1[h];
+                        val[h] = (q > 0.0f && val[h] > old) ? val[h] : old;
+                    }
             }
             if (p.vec_ok) {
                 __stcs(reinterpret_cast<float4 *>(oo), make_float4(val[0], val[1], val[2], val[3]));
@@ -1480,17 +1483,29 @@ __global__ void pt_order_kernel(long long n, const int *__restrict__ item_bucket
     order[bucket_start[b] + item_slot[a]] = (unsigned)a;
 }
 
+// Below SIGMA_EXACT the reference's own float64 result, 1 - exp(-x^12), is quantised to multiples of 2^-53 (exactly 0
+// for x^12 < 2^-54): at d -> 5 A and sigma = 0.7 A, x^12 = (0.14)^12 = 5.7e-11, so the quantisation is already 1e-6 of
+// the value, and it grows as sigma^-12 below that.  A float32 evaluation of the exact function cannot reproduce it; the
+// points kernel evaluates such channels with the reference's float64 operations instead (s2 < 0 marks them); the grid
+// entry points zero them for the grid kernels and run this kernel on the grid centres (occupancy_utils.py).  Bit parity
+// with the reference there also needs the device's double exp to round like glibc's where x^12 is small and exp(-x^12)
+// lands within a few ulp of 1: not guaranteed by either library, it holds on every case of
+// tests/test_occupancy_contract_gpu.py::test_sigma_sweep.  The extra branch and the exact[] array cost every points call;
+// that cost is not measured by bench.py (grid workloads only).
+constexpr double SIGMA_EXACT = 0.7;
+
 __global__ void pt_sigma_kernel(const double *__restrict__ sigmas, long long n, float *__restrict__ s2) {
     const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (i >= n) return;
     const double s = sigmas[i];
-    s2[i] = (s == 0.0 || s != s) ? 0.0f : fmaxf((float)(s * s), FLT_MIN);
+    s2[i] = (s == 0.0 || s != s) ? 0.0f : (fabs(s) < SIGMA_EXACT ? -1.0f : fmaxf((float)(s * s), FLT_MIN));
 }
 
 template <int CP>
 __global__ void __launch_bounds__(128) occ_points_kernel(const double *__restrict__ centers, long long M,
                                                          const float *__restrict__ coords,
-                                                         const float *__restrict__ s2, int C, unsigned hmask,
+                                                         const float *__restrict__ s2, const double *__restrict__ sigmas,
+                                                         int C, unsigned hmask,
                                                          const unsigned *__restrict__ bucket_start,
                                                          const unsigned *__restrict__ order, float *__restrict__ out,
                                                          unsigned flags) {
@@ -1498,8 +1513,9 @@ __global__ void __launch_bounds__(128) occ_points_kernel(const double *__restric
     if (m >= M) return;
     const double cx = centers[3 * m], cy = centers[3 * m + 1], cz = centers[3 * m + 2];
     float acc[CP];
+    float exact[CP];  // max of the float64 values of the sigma < SIGMA_EXACT channels; -1: no such atom reached
 #pragma unroll
-    for (int h = 0; h < CP; ++h) acc[h] = 0.0f;
+    for (int h = 0; h < CP; ++h) { acc[h] = 0.0f; exact[h] = -1.0f; }
     if (fabs(cx) < PT_LIMIT && fabs(cy) < PT_LIMIT && fabs(cz) < PT_LIMIT) {
         const long long kx = (long long)floor(cx * (1.0 / CUTOFF_A)), ky = (long long)floor(cy * (1.0 / CUTOFF_A)),
                         kz = (long long)floor(cz * (1.0 / CUTOFF_A));
@@ -1516,8 +1532,19 @@ __global__ void __launch_bounds__(128) occ_points_kernel(const double *__restric
                     const float r = rcp_approx((float)d2);
                     const float *sa = s2 + (long long)a * C;
 #pragma unroll
-                    for (int h = 0; h < CP; ++h)
-                        if (h < C) acc[h] = fmaxf(acc[h], sa[h] * r);  // A^2/A^2: same q as the grid path
+                    for (int h = 0; h < CP; ++h) {
+                        if (h < C) {
+                            const float s = sa[h];
+                            if (s >= 0.0f) {
+                                acc[h] = fmaxf(acc[h], s * r);  // A^2/A^2: same q as the grid path
+                            } else {  // pyx:57-60 in the reference's order and precision
+                                const double x = sigmas[(long long)a * C + h] / sqrt(d2);
+                                const double x3 = (x * x) * x;
+                                const double x12 = ((x3 * x3) * x3) * x3;
+                                exact[h] = fmaxf(exact[h], (float)(1.0 - exp(-x12)));
+                            }
+                        }
+                    }
                 }
             }
         }
@@ -1526,9 +1553,11 @@ __global__ void __launch_bounds__(128) occ_points_kernel(const double *__restric
 #pragma unroll
     for (int h = 0; h < CP; ++h) {
         if (h < C) {
-            float v = occ_value(acc[h]);
-            if (flags & MKB_OCC_ACCUMULATE) { const float old = o[h]; v = (v > old) ? v : old; }
-            o[h] = v;
+            const float v = fmaxf(occ_value(acc[h]), exact[h]);
+            // accumulate: only a voxel-channel some atom with a non-zero sigma reached is updated (pyx:56-61)
+            const bool reached = acc[h] > 0.0f || exact[h] >= 0.0f;
+            if (flags & MKB_OCC_ACCUMULATE) { const float old = o[h]; o[h] = (reached && v > old) ? v : old; }
+            else o[h] = v;
         }
     }
 }
@@ -2187,9 +2216,9 @@ extern "C" int mkb_occupancy_points(mkb_handle_t h, void *stream, const double *
         MKB_LAUNCHED(h);
     }
     const unsigned g2 = (unsigned)cdiv(M, 128);
-    if (C <= 8) occ_points_kernel<8><<<g2, 128, 0, st>>>(centers, M, coords, s2, C, hmask, bstart, order, out, flags);
-    else if (C <= 16) occ_points_kernel<16><<<g2, 128, 0, st>>>(centers, M, coords, s2, C, hmask, bstart, order, out, flags);
-    else occ_points_kernel<32><<<g2, 128, 0, st>>>(centers, M, coords, s2, C, hmask, bstart, order, out, flags);
+    if (C <= 8) occ_points_kernel<8><<<g2, 128, 0, st>>>(centers, M, coords, s2, sigmas, C, hmask, bstart, order, out, flags);
+    else if (C <= 16) occ_points_kernel<16><<<g2, 128, 0, st>>>(centers, M, coords, s2, sigmas, C, hmask, bstart, order, out, flags);
+    else occ_points_kernel<32><<<g2, 128, 0, st>>>(centers, M, coords, s2, sigmas, C, hmask, bstart, order, out, flags);
     MKB_LAUNCHED(h);
     return MKB_OK;
 }

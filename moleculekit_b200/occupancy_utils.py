@@ -14,6 +14,10 @@ import torch
 from . import _lib
 
 MAX_CHANNELS_PER_CALL = 32
+# Channel sigmas with 0 < |sigma| < SIGMA_EXACT (Angstrom) are evaluated with the reference's float64 operations by the
+# points kernel (SIGMA_EXACT in csrc/occupancy.cu, DESIGN.md K1b): there the reference's own 1 - exp(-x^12) is quantised
+# to multiples of 2^-53, which no float32 evaluation reproduces.
+SIGMA_EXACT = 0.7
 
 
 def _dev(device) -> torch.device:
@@ -69,13 +73,70 @@ def _layout_flag(layout: str) -> int:
     raise ValueError("layout must be 'xyzc' (the reference's voxel-major order) or 'cxyz' (channel-major)")
 
 
+def split_small_sigmas(sigmas: torch.Tensor | None, radii: torch.Tensor | None = None, chanmask: torch.Tensor | None = None,
+                       n_channels: int | None = None):
+    """None when no channel entry has 0 < |sigma| < SIGMA_EXACT; else (the sigmas -- or radii -- with those entries zeroed,
+    for the grid kernels; an (N, C) float64 matrix holding only those entries).  With bit-mask channels a small radius
+    moves the whole atom.  Reads one flag back to the host (synchronises torch's current stream)."""
+    if sigmas is not None:
+        small = (sigmas != 0) & (sigmas.abs() < SIGMA_EXACT)
+        if not bool(small.any()):
+            return None
+        return sigmas.masked_fill(small, 0.0), torch.where(small, sigmas, torch.zeros_like(sigmas))
+    Cn = int(n_channels)
+    bits = ((chanmask[:, None] >> torch.arange(Cn, device=chanmask.device, dtype=torch.int32)) & 1).bool()
+    atom = (radii != 0) & (radii.abs() < SIGMA_EXACT) & bits.any(dim=1)
+    if not bool(atom.any()):
+        return None
+    small = bits & atom[:, None]
+    return radii.masked_fill(atom, 0.0), torch.where(small, radii[:, None].expand(-1, Cn), torch.zeros((), dtype=radii.dtype, device=radii.device))
+
+
+def _merge_small_sigmas(coords: torch.Tensor, small: torch.Tensor, descs: np.ndarray, out: torch.Tensor, layout: str) -> None:
+    """Max-merge the float64 small-sigma values (points kernel on each grid's centres and own atoms) into the grid output;
+    entries no small-sigma atom reaches keep their bits."""
+    Cn = int(small.shape[1])
+    descs = np.ascontiguousarray(descs, dtype=_lib.GRID_DESC)
+    has = np.concatenate([[0], np.cumsum(small.ne(0).any(dim=1).cpu().numpy())])
+    flat = out.view(-1)
+    for b in range(len(descs)):
+        d = descs[b:b + 1].copy()
+        a0, a1 = int(d["atom_begin"][0]), int(d["atom_end"][0])
+        if has[a1] == has[a0]:
+            continue
+        M = int(np.prod(d["dims"][0]))
+        o = int(d["out_offset"][0]) * Cn
+        d["out_offset"] = 0
+        val = torch.full((M, Cn), float("-inf"), dtype=torch.float32, device=out.device)
+        occupancy_points(grid_centers(d, out.device), coords[a0:a1], small[a0:a1].contiguous(), val, accumulate=True)
+        g = flat[o:o + M * Cn].view(M, Cn) if layout == "xyzc" else flat[o:o + M * Cn].view(Cn, M).t()
+        g.copy_(torch.where(val > g, val, g))
+
+
 def occupancy_grid_batch(coords: torch.Tensor, sigmas: torch.Tensor | None, descs: np.ndarray, out: torch.Tensor,
                          accumulate: bool = False, layout: str = "xyzc", radii: torch.Tensor | None = None,
-                         chanmask: torch.Tensor | None = None, n_channels: int | None = None) -> torch.Tensor:
+                         chanmask: torch.Tensor | None = None, n_channels: int | None = None,
+                         small_sigmas: bool | None = None) -> torch.Tensor:
     """Launch K2+K1 for a batch of regular grids.  coords (N,3) f32 cuda, out (sum M_b * C) f32 cuda (written in place),
     channels either as ``sigmas`` (N,C) f64 cuda -- the reference's matrix -- or, assembled on the device, as ``radii``
     (N,) f64 + ``chanmask`` (N,) int32 bit masks with ``n_channels`` (SURVEY 8f row 1).  ``layout="cxyz"`` stores every grid
-    channel-major, [C][nx][ny][nz].  Stream-ordered on torch's current stream."""
+    channel-major, [C][nx][ny][nz].  Stream-ordered on torch's current stream.
+
+    Channel entries with 0 < |sigma| < SIGMA_EXACT are zeroed in the copy the grid kernels see and evaluated in float64 by
+    the points kernel on the grid centres, then max-merged.  ``small_sigmas=False`` is the caller's word that there are
+    none (no check, no host synchronisation: the batch takes the grid kernels alone); None checks on the device."""
+    split = None
+    if small_sigmas is not False:
+        split = split_small_sigmas(sigmas, radii, chanmask, n_channels if sigmas is None else None)
+    if split is not None:
+        fast, small = split
+        if sigmas is not None:
+            occupancy_grid_batch(coords, fast, descs, out, accumulate, layout, small_sigmas=False)
+        else:
+            occupancy_grid_batch(coords, None, descs, out, accumulate, layout, radii=fast, chanmask=chanmask,
+                                 n_channels=n_channels, small_sigmas=False)
+        _merge_small_sigmas(coords, small, descs, out, layout)
+        return out
     dev = out.device
     assert coords.is_cuda and out.is_cuda and coords.device == dev
     assert coords.dtype == torch.float32 and out.dtype == torch.float32
@@ -112,11 +173,14 @@ def occupancy_grid_batch(coords: torch.Tensor, sigmas: torch.Tensor | None, desc
 
 def occupancy_grid_batch_compact(coords: torch.Tensor, sigmas: torch.Tensor | None, descs: np.ndarray,
                                  radii: torch.Tensor | None = None, chanmask: torch.Tensor | None = None,
-                                 records: torch.Tensor | None = None, blk_rank: torch.Tensor | None = None):
+                                 records: torch.Tensor | None = None, blk_rank: torch.Tensor | None = None,
+                                 small_sigmas: bool | None = None):
     """K2+K1 with the compact result of ``mkb_occupancy_grid_batch_compact`` (8 channels): returns (records, blk_rank),
     ``records`` float32 cuda with one 4 KB row [4 x][4 y][8 z][8 ch] per 4x4x8-voxel block that has an atom within 5 A
     (room for every block of the batch; only the first blk_rank[-1] rows are written) and ``blk_rank`` int32 (blocks + 1,)
     the exclusive count of such blocks.  :func:`expand_compact_host` rebuilds the dense host array."""
+    if small_sigmas is not False and split_small_sigmas(sigmas, radii, chanmask, 8 if sigmas is None else None) is not None:
+        raise _lib.MkbUnsupported("channel sigmas below SIGMA_EXACT need the dense route (occupancy_grid_batch)")
     dev = coords.device
     assert coords.is_cuda and coords.dtype == torch.float32 and coords.is_contiguous() and coords.ndim == 2
     descs = np.ascontiguousarray(descs, dtype=_lib.GRID_DESC)
@@ -145,11 +209,14 @@ def occupancy_grid_batch_compact(coords: torch.Tensor, sigmas: torch.Tensor | No
 
 
 def occupancy_grid_batch_to_host(coords: torch.Tensor, sigmas: torch.Tensor | None, descs: np.ndarray, out_host: torch.Tensor,
-                                 radii: torch.Tensor | None = None, chanmask: torch.Tensor | None = None):
+                                 radii: torch.Tensor | None = None, chanmask: torch.Tensor | None = None,
+                                 small_sigmas: bool | None = None):
     """K2+K1 storing the non-empty 4x4x8 blocks straight into ``out_host`` -- a PINNED host float32 tensor (sum M, 8), device
     accessible under UVA -- while the block index travels to the host ahead of the fill kernel
     (``mkb_occupancy_grid_batch_to_host``).  Returns the pinned int32 index (blocks + 1,); call :func:`wait_index`, zero-fill
     the empty blocks with :func:`expand_compact_host` (``records=None``) and synchronise the stream before reading."""
+    if small_sigmas is not False and split_small_sigmas(sigmas, radii, chanmask, 8 if sigmas is None else None) is not None:
+        raise _lib.MkbUnsupported("channel sigmas below SIGMA_EXACT need the dense route (occupancy_grid_batch)")
     dev = coords.device
     assert coords.is_cuda and coords.dtype == torch.float32 and coords.is_contiguous() and coords.ndim == 2
     assert not out_host.is_cuda and out_host.is_pinned() and out_host.dtype == torch.float32 and out_host.is_contiguous()
@@ -301,8 +368,10 @@ def calculate_occupancy(centers, coords, sigmas, results, device=None) -> None:
     d_coords = torch.from_numpy(np.ascontiguousarray(coords)).to(dev)
     for c0, c1 in _channel_chunks(Cn):
         d_sig = torch.from_numpy(np.ascontiguousarray(sigmas[:, c0:c1])).to(dev)
-        d_out = torch.empty((M, c1 - c0), dtype=torch.float32, device=dev)
-        occupancy_points(d_centers, d_coords, d_sig, d_out)
+        # -inf marks the entries no atom with a non-zero sigma reached: the reference leaves those untouched, whatever
+        # `results` holds there (a negative prefill included)
+        d_out = torch.full((M, c1 - c0), float("-inf"), dtype=torch.float32, device=dev)
+        occupancy_points(d_centers, d_coords, d_sig, d_out, accumulate=True)
         val = d_out.cpu().numpy().astype(np.float64)
         old = results[:M, c0:c1]
         # reference update rule `value > old ? value : old` (NaN in `old` sticks, never produced by us)

@@ -348,10 +348,25 @@ class VoxelBatch:
         (rows [out_offsets[b], out_offsets[b+1])) holds that grid channel-major, see :meth:`as_cxyz`."""
         if out is None:
             out = torch.empty((self.total_voxels, self.C), dtype=torch.float32, device=d_coords.device)
+        small = None if self.has_small_sigmas(d_channels) else False
         if isinstance(d_channels, tuple):
             return _occ.occupancy_grid_batch(d_coords, None, self.descs, out, layout=layout, radii=d_channels[0],
-                                             chanmask=d_channels[1], n_channels=self.C)
-        return _occ.occupancy_grid_batch(d_coords, d_channels, self.descs, out, layout=layout)
+                                             chanmask=d_channels[1], n_channels=self.C, small_sigmas=small)
+        return _occ.occupancy_grid_batch(d_coords, d_channels, self.descs, out, layout=layout, small_sigmas=small)
+
+    def has_small_sigmas(self, d_channels) -> bool:
+        """Whether some channel entry has 0 < |sigma| < occupancy_utils.SIGMA_EXACT (evaluated in float64 after the grid
+        kernels).  Checked on the device once per channel tensor and remembered, so repeated runs on resident inputs
+        never wait for the stream."""
+        t = d_channels if isinstance(d_channels, tuple) else (d_channels,)
+        key = tuple((x.data_ptr(), x.numel()) for x in t)
+        if getattr(self, "_small_key", None) != key:
+            if isinstance(d_channels, tuple):
+                split = _occ.split_small_sigmas(None, d_channels[0], d_channels[1], self.C)
+            else:
+                split = _occ.split_small_sigmas(d_channels)
+            self._small_key, self._small = key, split is not None
+        return self._small
 
     def rotate(self, d_coords, rotations, rot_centers) -> torch.Tensor:
         """Random-rotation augmentation on the device: item b is rotated by rotations[b] = [rx, ry, rz] about
@@ -394,9 +409,11 @@ def _direct_to_host(batch, d_coords, d_chan, dev, out):
     index reaches the host before the fill kernel starts."""
     t_out = torch.from_numpy(out)
     if isinstance(d_chan, tuple):
-        h_rank_t, _keep = _occ.occupancy_grid_batch_to_host(d_coords, None, batch.descs, t_out, radii=d_chan[0], chanmask=d_chan[1])
+        h_rank_t, _keep = _occ.occupancy_grid_batch_to_host(d_coords, None, batch.descs, t_out, radii=d_chan[0], chanmask=d_chan[1],
+                                                                small_sigmas=batch.has_small_sigmas(d_chan))
     else:
-        h_rank_t, _keep = _occ.occupancy_grid_batch_to_host(d_coords, d_chan, batch.descs, t_out)
+        h_rank_t, _keep = _occ.occupancy_grid_batch_to_host(d_coords, d_chan, batch.descs, t_out,
+                                                                small_sigmas=batch.has_small_sigmas(d_chan))
     _occ.wait_index(dev)
     h_rank = h_rank_t.numpy()
     _occ.expand_compact_host(batch.descs, 0, batch.B, h_rank, None, 0, out)   # zeros for the blocks the GPU does not write
@@ -409,9 +426,10 @@ def _direct_to_host(batch, d_coords, d_chan, dev, out):
 def _compact_to_host(batch, d_coords, d_chan, dev, out, dtype, n_chunks: int = 0):
     """Compact transfer: block records + index over PCIe in chunks, dense array rebuilt by host threads meanwhile."""
     if isinstance(d_chan, tuple):
-        recs, rank = _occ.occupancy_grid_batch_compact(d_coords, None, batch.descs, radii=d_chan[0], chanmask=d_chan[1])
+        recs, rank = _occ.occupancy_grid_batch_compact(d_coords, None, batch.descs, radii=d_chan[0], chanmask=d_chan[1],
+                                                         small_sigmas=batch.has_small_sigmas(d_chan))
     else:
-        recs, rank = _occ.occupancy_grid_batch_compact(d_coords, d_chan, batch.descs)
+        recs, rank = _occ.occupancy_grid_batch_compact(d_coords, d_chan, batch.descs, small_sigmas=batch.has_small_sigmas(d_chan))
     cur = torch.cuda.current_stream(dev)
     h_rank_t = torch.empty(rank.shape, dtype=torch.int32, pin_memory=True)
     h_rank_t.copy_(rank, non_blocking=True)

@@ -99,10 +99,11 @@ def test_calculate_occupancy_accumulates(oracle):
     ctr = rng.normal(size=(900, 3)) * 5
     sg = rng.choice([0.0, 1.2, 1.7], size=(64, 5))
     sg[3, 1] = np.nan
-    want = np.full((900, 5), 0.25); oracle.calculate_occupancy(ctr, xyz, sg, want)
-    got = np.full((900, 5), 0.25); calculate_occupancy(ctr, xyz, sg, got)
-    assert np.allclose(got, want, rtol=RTOL, atol=0)
-    assert np.array_equal(got == 0.25, want == 0.25)
+    for fill in (0.25, -1.0, -np.inf):  # a negative prefill stays wherever no atom with a non-zero sigma reaches
+        want = np.full((900, 5), fill); oracle.calculate_occupancy(ctr, xyz, sg, want)
+        got = np.full((900, 5), fill); calculate_occupancy(ctr, xyz, sg, got)
+        assert np.allclose(got, want, rtol=RTOL, atol=0)
+        assert np.array_equal(got == fill, want == fill)
     with pytest.raises(ValueError):
         calculate_occupancy(ctr.astype(np.float32), xyz, sg, got)
 
