@@ -58,7 +58,7 @@ def build(force: bool = False, verbose: bool = True, extra: list[str] | None = N
     if not force and not _stale():
         return LIB
     os.makedirs(LIBDIR, exist_ok=True)
-    env_extra = os.environ.get("MKB_NVCC_EXTRA", "").split()  # e.g. -DMKB_W_MIN_CTAS=12 for tuning experiments
+    env_extra = os.environ.get("MKB_NVCC_EXTRA", "").split()  # e.g. -DMKB_R_MIN_CTAS=4 for tuning experiments
     cmd = [nvcc_path()] + NVCC_FLAGS + (extra or []) + env_extra + [f"-I{INCLUDE}", f"-I{CSRC}", "-o", LIB] + sources()
     if verbose:
         print("[mkb200 build]", " ".join(cmd), flush=True)

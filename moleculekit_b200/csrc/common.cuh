@@ -25,7 +25,7 @@ enum ScratchSlot {
     S_PT_ORDER,     // points path: atom order
     S_ROWCNT,       // contacts: per-row counts
     S_COM,          // reductions: centres of mass
-    S_TILE_TOTAL,   // occupancy fast paths: halo atom count per tile / per block
+    S_TILE_TOTAL,   // occupancy warp kernel: halo atom count per block
     S_BLOCK_BASE,   // occupancy warp kernel: first block id of every grid
     S_K4_BALLOTS,   // contacts: hit masks of the count pass, reused by the fill pass
     S_BAND_BITMAP,  // occupancy run kernel: one bit per voxel whose gate decision is re-done in float64

@@ -7,11 +7,17 @@
 //   value(c,h) = max_a [ d2 < 25 ] (1 - exp(-(sigma_ah^2/d2)^6)).   f(q) = 1 - exp(-q^6) is monotone in
 //   q = sigma^2/d2, so the max over atoms commutes with f: the hot loop only tracks max q per voxel-channel and the
 //   transcendental runs ONCE per voxel-channel in the epilogue.
-//   K2  bin atoms of every grid of the batch into 8-voxel cells (count -> cub scan -> scatter), positions kept as
-//       float64 voxel coordinates p' = (x - origin)/voxelsize.
-//   K1  one CTA (512 threads) per 8x8x8-voxel tile: gather the tile's halo atoms from <= (R+1)^2 contiguous cell rows
-//       into shared memory as float positions RELATIVE TO THE TILE CORNER (|rel| < 32, so fp32 keeps ~5e-7 voxel
-//       absolute accuracy wherever the molecule sits), then each warp owns a 2x4x4 voxel block, culls the list
+//   K1  three fill kernels; occupancy_grid_batch_impl picks one per call from the input alone:
+//       occ_fill_runs_kernel (occ_runs.cuh, fed by its own block lists K2'): 8 channels, no accumulate, 16-byte aligned
+//         output, cutoff <= 40 voxels -- the default;
+//       occ_fill8v_kernel: the other calls with <= 8 channels and a cutoff <= 14 voxels, one warp per 2x4x8 block;
+//       occ_fill_kernel<CP>: everything else (9..32 channels, finer grids, or the 15..40-voxel cutoffs the run kernel
+//         does not serve), described below.
+//   K2  bin atoms of every grid of the batch into cells (count -> cub scan -> scatter): 4 voxels for occ_fill8v_kernel,
+//       8 otherwise; positions kept as float64 voxel coordinates p' = (x - origin)/voxelsize.
+//   occ_fill_kernel: one CTA (512 threads) per 8x8x8-voxel tile: gather the tile's halo atoms from <= (R+1)^2 contiguous
+//       cell rows into shared memory as float positions RELATIVE TO THE TILE CORNER (|rel| < 32, so fp32 keeps ~5e-7
+//       voxel absolute accuracy wherever the molecule sits), then each warp owns a 2x4x4 voxel block, culls the list
 //       against its block with one ballot per 32 atoms and accumulates max q in registers (8 channels = 8 FMNMX).
 //       Pairs whose d2 falls within 4e-6 (relative) of the 5 A gate are re-evaluated in float64 with the reference's
 //       exact operation order, so the discontinuity at the gate is reproduced bit-for-bit.
@@ -66,22 +72,14 @@ __device__ __forceinline__ float ex2_approx(float x) {
     return r;
 }
 
-#ifndef MKB_VALUE_SHORT
-#define MKB_VALUE_SHORT 1
-#endif
 // 1 - exp(-q^6), q = sigma^2/d2  (== 1 - exp(-(sigma/r)^12), occupancy_utils.pyx:57-60), relative error ~1e-6.
 __device__ __forceinline__ float occ_value(float q) {
     const float q2 = q * q;
     const float q3 = q2 * q;
     const float t = q3 * q3;
     // small t: -expm1(-t) by Taylor (avoids the cancellation that costs 0.4 relative error in naive fp32)
-#if MKB_VALUE_SHORT
     // below t = 0.25 the t^6 / 5040 term is 4.8e-8 of the value: under half a float ulp
     float s = fmaf(t, -1.0f / 720.0f, 1.0f / 120.0f);
-#else
-    float s = fmaf(t, 1.0f / 5040.0f, -1.0f / 720.0f);
-    s = fmaf(t, s, 1.0f / 120.0f);
-#endif
     s = fmaf(t, s, -1.0f / 24.0f);
     s = fmaf(t, s, 1.0f / 6.0f);
     s = fmaf(t, s, -0.5f);
@@ -96,14 +94,6 @@ __device__ __forceinline__ int find_grid_item(const GridDev *g, int B, long long
     while (lo < hi) {
         const int mid = (lo + hi + 1) >> 1;
         if (g[mid].item_base <= v) lo = mid; else hi = mid - 1;
-    }
-    return lo;
-}
-__device__ __forceinline__ int find_grid_tile(const GridDev *g, int B, long long v) {
-    int lo = 0, hi = B - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (g[mid].tile_base <= v) lo = mid; else hi = mid - 1;
     }
     return lo;
 }
@@ -209,8 +199,7 @@ struct FillParams {
     unsigned flags;
     int vec_ok;
     int cmajor;     // MKB_OCC_LAYOUT_CXYZ: grid b is stored [C][nx][ny][nz] (channel-major) instead of [nx][ny][nz][C]
-    int txp_shift;  // fast path launch: blockIdx.z = (grid << txp_shift) | tile_x
-    int bulk_store; // fast path: stage the tile in smem and store rows with cp.async.bulk (TMA)
+    int txp_shift;  // warp kernel launch: blockIdx.z = (grid << txp_shift) | block_x
     // warp kernel, uniform launches: descriptor of the chunk's first grid + per-grid strides
     GridDev u;
     long long u_out_stride, u_cell_stride, u_block_base, u_block_stride;
@@ -458,373 +447,39 @@ __global__ void __launch_bounds__(FILL_THREADS, (CP <= 8 ? 2 : 1)) occ_fill_kern
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// K1 fast path (C <= 8): quarter-warp candidate lists.
-//   The 2x4x4 block of a warp is split into four 2x2x2 sub-blocks, one per quarter-warp (8 lanes).  An atom within
-//   5 A of the 2x4x4 block is within 5 A of only ~66 % of the voxels of a 2x2x2 sub-block it touches (43 % for the
-//   whole block), so giving every quarter its OWN compacted candidate list removes a third of the wasted lane work.
-//   Lists hold 16-bit indices into the tile list; LDS.128 serves the four quarters' four different records in its four
-//   phases at no extra cost.  Shorter quarters are padded with a far-away sentinel so the loop stays branch-free.
+// K1 v6 (C <= 8 channels, cutoff <= 14 voxels, calls the run kernel does not serve): no CTA-level synchronisation.
+//   Each warp owns one 2x4x8 voxel block end to end: it gathers the block's own halo from 4-voxel cells (<= 64 contiguous
+//   cell rows) into its private shared-memory list, splits it into eight 2x2x2 sub-block lists (sy in 0..1, sz in 0..3,
+//   four lanes each) and runs them in lock-step; empty blocks retire after one halo count.  A lane owns the x-pair of
+//   voxels (0, y, z) and (1, y, z).  Against one voxel per lane on 2x4x4 blocks:
+//     * one halo gather (cell rows are contiguous along z, so doubling the block along z adds ~20 % scanned atoms, not
+//       100 %), one row set-up, one prologue per 64 voxels instead of per 32;
+//     * a candidate is loaded once for two voxels that share dy, dz and the channel mask: 39 instructions per candidate
+//       for two pairs instead of 30 for one, while each 2x2x2 sub-block keeps its own list (same 47 % hit rate);
+//     * two independent dependency chains per lane (ILP) stand in for the halved number of resident warps.
 // ---------------------------------------------------------------------------------------------------------
+constexpr int V_CELL = 4;     // cell edge of the binning used with this kernel
+constexpr int V_ROWS = 64;    // cell rows per block: (Rx+1)(Ry+1) <= 64 up to a 14-voxel cutoff
+constexpr int V_BZ = 8;       // block extent along z
+// capacity sweep (ms per 256 pockets): 128/96 1.864, 160/96 1.858, 224/96 1.841, 192/128 1.814, 224/128 1.825, 256/128 1.850
+constexpr int V_PCAP = 192;   // block candidates per round
+constexpr int V_QCAP = 128;   // sub-block candidates per round
+constexpr int V_QSTRIDE = V_QCAP + 2;  // + one sentinel slot for the software-pipelined loop
+constexpr int V_WARPS = 1;    // warps (= blocks) per CTA. A CTA holds its registers until its slowest warp retires
+constexpr int V_MIN_CTAS = 7; // 72 registers; at 8 CTAs (64 registers) the kernel spills
 constexpr float GATE_SCALE = 1.2676506002282294e30f;  // 2^100
-constexpr int V3_CAP = 1024;   // tile list (halo atoms of one 8x8x8 tile) per pass
-constexpr int V3_PCAP = 160;   // parent (2x4x4 block) candidates per round
-constexpr int V3_QCAP = 96;    // sub-block (2x2x2) candidates per round
 
-__global__ void occ_tile_total_kernel(const GridDev *__restrict__ grids, const unsigned *__restrict__ cell_start,
-                                      unsigned *__restrict__ tile_total) {
+__global__ void occ_block_total_v_kernel(const GridDev *__restrict__ grids, const unsigned *__restrict__ cell_start,
+                                         const long long *__restrict__ block_base, unsigned *__restrict__ block_total) {
     const GridDev &g = grids[blockIdx.y];
-    const int ntiles = g.tiles[0] * g.tiles[1] * g.tiles[2];
-    const int local = blockIdx.x * blockDim.x + threadIdx.x;
-    if (local >= ntiles) return;
-    const int tzN = g.tiles[2], tyN = g.tiles[1];
-    const int tz = local % tzN, txy = local / tzN, ty = txy % tyN, tx = txy / tyN;
-    const int R = g.rcells, cN1 = g.cells[1], cN2 = g.cells[2];
-    const int cx1 = min(tx + R, g.cells[0] - 1), cy1 = min(ty + R, cN1 - 1), cz1 = min(tz + R, cN2 - 1);
-    unsigned total = 0;
-    for (int cx = tx; cx <= cx1; ++cx)
-        for (int cy = ty; cy <= cy1; ++cy) {
-            const long long cb = g.cell_base + ((long long)cx * cN1 + cy) * cN2;
-            total += cell_start[cb + cz1 + 1] - cell_start[cb + tz];
-        }
-    tile_total[g.tile_base + local] = total;
-}
-
-__global__ void __launch_bounds__(FILL_THREADS, 2) occ_fill8_kernel(const FillParams p, const unsigned *__restrict__ tile_total) {
-    __shared__ float4 s_ent[V3_CAP + 1];  // +1: sentinel
-    __shared__ unsigned s_mask[V3_CAP + 1];
-    __shared__ unsigned s_src[V3_CAP];
-    __shared__ unsigned s_rpos[128];
-    __shared__ unsigned s_rbase[128 + 1];
-    __shared__ unsigned short s_pidx[FILL_THREADS / 32][V3_PCAP];
-    __shared__ unsigned short s_qidx[FILL_THREADS / 32][4][V3_QCAP];
-    __shared__ int s_cnt;
-
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    // grid = (tiles_z, tiles_y, grids << txp_shift | tiles_x): no integer division in the prologue
-    const int tz = blockIdx.x, ty = blockIdx.y, tx = blockIdx.z & ((1 << p.txp_shift) - 1);
-    const GridDev *gg = p.grids + (blockIdx.z >> p.txp_shift);
-    const int tzN = __ldg(&gg->tiles[2]), tyN = __ldg(&gg->tiles[1]);
-    if (tz >= tzN || ty >= tyN || tx >= __ldg(&gg->tiles[0])) return;  // ragged batch / power-of-two padding
-    const int local = (tx * tyN + ty) * tzN + tz;
-    const int nx = __ldg(&gg->dims[0]), ny = __ldg(&gg->dims[1]), nz = __ldg(&gg->dims[2]);
-    const unsigned total = __ldg(tile_total + __ldg(&gg->tile_base) + local);
-
-    // ---- empty tile (3 of 4 tiles in a typical pocket grid): stream the zeros with minimal index math and retire
-    if (total == 0 && p.vec_ok && !(p.flags & MKB_OCC_ACCUMULATE)) {
-        const int row = tid >> 3, izz = tz * TILE + (tid & 7);  // 8 consecutive threads = one 256-byte row
-        const int ixr = tx * TILE + (row >> 3), iyr = ty * TILE + (row & 7);
-        if (ixr < nx && iyr < ny && izz < nz) {
-            float4 *d = reinterpret_cast<float4 *>(p.out + (__ldg(&gg->out_offset) + ((long long)ixr * ny + iyr) * nz + izz) * 8);
-            const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            __stcs(d, z4);
-            __stcs(d + 1, z4);
-        }
-        return;
-    }
-
-    // lane -> voxel: quarter q = lane >> 3 owns the 2x2x2 sub-block (qy, qz) of the warp's 2x4x4 block
-    const int bx = warp >> 2, by = (warp >> 1) & 1, bz = warp & 1;
-    const int q = lane >> 3, sub = lane & 7;
-    const int vx = bx * 2 + (sub >> 2), vy = by * 4 + (q >> 1) * 2 + ((sub >> 1) & 1), vz = bz * 4 + (q & 1) * 2 + (sub & 1);
-    const int ix = tx * TILE + vx, iy = ty * TILE + vy, iz = tz * TILE + vz;
-    const bool inside = ix < nx && iy < ny && iz < nz;
-    float *const o = p.out + (__ldg(&gg->out_offset) + ((long long)ix * ny + iy) * nz + iz) * 8;
-
-    float acc[8];
-#pragma unroll
-    for (int h = 0; h < 8; ++h) acc[h] = 0.0f;
-    bool touched = false;
-
-    if (total != 0) {
-        // ---- cell rows feeding this tile (same scheme as the generic kernel)
-        const int R = __ldg(&gg->rcells);
-        const int cN1 = __ldg(&gg->cells[1]), cN2 = __ldg(&gg->cells[2]);
-        const int cx1 = min(tx + R, __ldg(&gg->cells[0]) - 1), cy1 = min(ty + R, cN1 - 1), cz1 = min(tz + R, cN2 - 1);
-        const int ncy = cy1 - ty + 1;
-        const int nrows = (cx1 - tx + 1) * ncy;  // <= 128 checked on the host
-        if (tid < nrows) {
-            const int rx = tid / ncy, ry = tid - rx * ncy;
-            const long long cb = __ldg(&gg->cell_base) + ((long long)(tx + rx) * cN1 + (ty + ry)) * cN2;
-            const unsigned a = __ldg(p.cell_start + cb + tz), e = __ldg(p.cell_start + cb + cz1 + 1);
-            s_rpos[tid] = a;
-            s_rbase[tid + 1] = e - a;
-        }
-        if (tid == 0) {
-            s_rbase[0] = 0;
-            s_cnt = 0;
-            s_ent[V3_CAP] = make_float4(1e18f, 1e18f, 1e18f, 0.0f);  // sentinel: never inside the gate
-            s_mask[V3_CAP] = 1u;
-        }
-        __syncthreads();
-        if (warp == 0) {
-            unsigned carry = 0;
-            for (int c0 = 0; c0 < nrows; c0 += 32) {
-                const int r = c0 + lane;
-                unsigned v = (r < nrows) ? s_rbase[r + 1] : 0u;
-#pragma unroll
-                for (int s = 1; s < 32; s <<= 1) {
-                    const unsigned t = __shfl_up_sync(0xffffffffu, v, s);
-                    if (lane >= s) v += t;
-                }
-                if (r < nrows) s_rbase[r + 1] = v + carry;
-                carry += __shfl_sync(0xffffffffu, v, 31);
-            }
-        }
-        __syncthreads();
-
-        const float cut_lo = __ldg(&gg->cut2v_lo), cut_hi = __ldg(&gg->cut2v_hi);
-        const float gate_k = GATE_SCALE * cut_lo;  // exact: power-of-two scaling
-        const unsigned band_bits = __float_as_uint(cut_hi - cut_lo);
-        // tile frame: origin at the tile CENTRE (voxel 3.5), so |coordinate| <= 3.5 + cutv and fp32 spacing is finest
-        const float fvx = (float)vx - TILE_C, fvy = (float)vy - TILE_C, fvz = (float)vz - TILE_C;
-        const float bcx = (float)(bx * 2) - TILE_C, bcy = (float)(by * 4) - TILE_C, bcz = (float)(bz * 4) - TILE_C;
-        unsigned short *const my_p = s_pidx[warp];
-        unsigned short *const my_q = s_qidx[warp][q];
-        unsigned ent_sa, mask_sa;  // taken once; volatile so ptxas does not rebuild them from SR_CgaCtaId per use
-        asm volatile("{ .reg .u64 t; cvta.to.shared.u64 t, %1; cvt.u32.u64 %0, t; }" : "=r"(ent_sa) : "l"(s_ent));
-        asm volatile("{ .reg .u64 t; cvta.to.shared.u64 t, %1; cvt.u32.u64 %0, t; }" : "=r"(mask_sa) : "l"(s_mask));
-
-        for (unsigned c0 = 0; c0 < total; c0 += V3_CAP) {  // one pass unless > V3_CAP atoms sit in the halo
-            if (c0) {
-                __syncthreads();
-                if (tid == 0) s_cnt = 0;
-                __syncthreads();
-            }
-            const unsigned c1 = min(total, c0 + (unsigned)V3_CAP);
-            {
-                const int cutv = __ldg(&gg->cutv);
-                const int cshift_x = tx * TILE + cutv, cshift_y = ty * TILE + cutv, cshift_z = tz * TILE + cutv;
-                for (unsigned k0 = c0; k0 < c1; k0 += FILL_THREADS) {
-                    const unsigned k = k0 + tid;
-                    bool pass = false;
-                    float4 e = make_float4(0.f, 0.f, 0.f, 0.f);
-                    unsigned m = 0, sr = 0;
-                    if (k < c1) {
-                        int lo = 0, hi = nrows - 1;
-                        while (lo < hi) {
-                            const int mid = (lo + hi + 1) >> 1;
-                            if (s_rbase[mid] <= k) lo = mid; else hi = mid - 1;
-                        }
-                        const unsigned i = s_rpos[lo] + (k - s_rbase[lo]);
-                        e = __ldg(p.rec_pos + i);
-                        const uint4 tg = __ldg(p.rec_tag + i);
-                        m = tg.x;
-                        sr = tg.y;
-                        e.x += (float)((int)(tg.z & 1023u) * TILE - cshift_x) - TILE_C;  // exact: small integers
-                        e.y += (float)((int)((tg.z >> 10) & 1023u) * TILE - cshift_y) - TILE_C;
-                        e.z += (float)((int)(tg.z >> 20) * TILE - cshift_z) - TILE_C;
-                        const float ddx = fmaxf(fabsf(e.x) - TILE_C, 0.f);
-                        const float ddy = fmaxf(fabsf(e.y) - TILE_C, 0.f);
-                        const float ddz = fmaxf(fabsf(e.z) - TILE_C, 0.f);
-                        pass = (m != 0) && (ddx * ddx + ddy * ddy + ddz * ddz <= cut_hi);
-                        if (sr & 0x80000000u) m = 0;  // several distinct sigmas: per-channel path
-                    }
-                    const unsigned bal = __ballot_sync(0xffffffffu, pass);
-                    if (bal) {
-                        int base = 0;
-                        if (lane == 0) base = atomicAdd(&s_cnt, __popc(bal));
-                        base = __shfl_sync(0xffffffffu, base, 0);
-                        if (pass) {
-                            const int slot = base + __popc(bal & ((1u << lane) - 1u));
-                            s_ent[slot] = e;
-                            s_mask[slot] = m;
-                            s_src[slot] = sr & 0x7fffffffu;
-                        }
-                    }
-                }
-            }
-            __syncthreads();
-            const int n = s_cnt;
-
-            int j0 = 0;
-            while (j0 < n) {
-                // ---- stage A: tile list -> indices of the atoms within reach of this warp's 2x4x4 block
-                int np = 0;
-                for (; j0 < n && np <= V3_PCAP - 32; j0 += 32) {
-                    const int j = j0 + lane;
-                    const float4 e = lds_f4(ent_sa + min(j, n - 1) * 16);
-                    const float rx = e.x - bcx, ry = e.y - bcy, rz = e.z - bcz;
-                    const float ddx = fmaxf(fmaxf(-rx, rx - 1.f), 0.f);
-                    const float ddy = fmaxf(fmaxf(-ry, ry - 3.f), 0.f);
-                    const float ddz = fmaxf(fmaxf(-rz, rz - 3.f), 0.f);
-                    const bool hit = (j < n) & (fmaf(ddz, ddz, fmaf(ddy, ddy, ddx * ddx)) <= cut_hi);
-                    const unsigned bal = __ballot_sync(0xffffffffu, hit);
-                    if (hit) my_p[np + __popc(bal & ((1u << lane) - 1u))] = (unsigned short)j;
-                    np += __popc(bal);
-                }
-                if (np == 0) continue;
-                touched = true;
-                __syncwarp();
-                // ---- stage B: parent list -> four sub-block lists; stage C: evaluate
-                int cq0 = 0, cq1 = 0, cq2 = 0, cq3 = 0;
-                for (int k0 = 0; k0 < np; k0 += 32) {
-                    const int k = k0 + lane;
-                    const bool live = k < np;
-                    const unsigned idx = my_p[min(k, np - 1)];
-                    bool h0, h1, h2, h3, multi;
-                    {
-                        const float4 e = lds_f4(ent_sa + idx * 16);
-                        const float rx = e.x - bcx, ry = e.y - bcy, rz = e.z - bcz;
-                        const float ddx = fmaxf(fmaxf(-rx, rx - 1.f), 0.f);
-                        const float y0 = fmaxf(fmaxf(-ry, ry - 1.f), 0.f), y1 = fmaxf(fmaxf(2.f - ry, ry - 3.f), 0.f);
-                        const float z0 = fmaxf(fmaxf(-rz, rz - 1.f), 0.f), z1 = fmaxf(fmaxf(2.f - rz, rz - 3.f), 0.f);
-                        const float xx = ddx * ddx;
-                        const float a0 = fmaf(y0, y0, xx), a1 = fmaf(y1, y1, xx);
-                        multi = live & (lds_u32(mask_sa + idx * 4) == 0);
-                        const bool ok = live & !multi;
-                        h0 = ok & (fmaf(z0, z0, a0) <= cut_hi);  // q = qy*2 + qz
-                        h1 = ok & (fmaf(z1, z1, a0) <= cut_hi);
-                        h2 = ok & (fmaf(z0, z0, a1) <= cut_hi);
-                        h3 = ok & (fmaf(z1, z1, a1) <= cut_hi);
-                    }
-                    // atoms carrying several distinct sigmas (user float channels): whole-warp per-channel path
-                    for (unsigned bm = __ballot_sync(0xffffffffu, multi); bm; bm &= bm - 1) {
-                        const int jj = my_p[k0 + __ffs(bm) - 1];
-                        const float4 e = s_ent[jj];
-                        const float dx = e.x - fvx, dy = e.y - fvy, dz = e.z - fvz;
-                        const float d2 = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-                        bool in = d2 < cut_lo;
-                        if (!in && d2 < cut_hi) in = exact_gate(gg, p.coords, s_src[jj], ix, iy, iz);
-                        const float rr = in ? rcp_approx(d2) : 0.0f;
-                        const double *sg = p.sigmas + (long long)s_src[jj] * p.C;
-                        const double ivs = __ldg(&gg->inv_vs);
-#pragma unroll
-                        for (int h = 0; h < 8; ++h) {
-                            if (h < p.C) {
-                                const double sv = sg[h] * ivs;
-                                const float sq = (sv == 0.0 || sv != sv) ? 0.0f : fmaxf((float)(sv * sv), FLT_MIN);
-                                acc[h] = fmaxf(acc[h], sq * rr);  // 0*inf = NaN is dropped by fmaxf
-                            }
-                        }
-                    }
-                    const unsigned lt = (1u << lane) - 1u;
-                    const unsigned b0 = __ballot_sync(0xffffffffu, h0), b1 = __ballot_sync(0xffffffffu, h1);
-                    const unsigned b2 = __ballot_sync(0xffffffffu, h2), b3 = __ballot_sync(0xffffffffu, h3);
-                    unsigned short *const wq = s_qidx[warp][0];
-                    if (h0) wq[0 * V3_QCAP + cq0 + __popc(b0 & lt)] = (unsigned short)idx;
-                    if (h1) wq[1 * V3_QCAP + cq1 + __popc(b1 & lt)] = (unsigned short)idx;
-                    if (h2) wq[2 * V3_QCAP + cq2 + __popc(b2 & lt)] = (unsigned short)idx;
-                    if (h3) wq[3 * V3_QCAP + cq3 + __popc(b3 & lt)] = (unsigned short)idx;
-                    cq0 += __popc(b0); cq1 += __popc(b1); cq2 += __popc(b2); cq3 += __popc(b3);
-                    const int nmax = max(max(cq0, cq1), max(cq2, cq3));
-                    if (k0 + 32 < np && nmax <= V3_QCAP - 32) continue;
-                    // pad the shorter quarters with the sentinel, then run all four lists in lock-step
-                    const int mine = (q == 0) ? cq0 : (q == 1) ? cq1 : (q == 2) ? cq2 : cq3;
-                    for (int c = mine + sub; c < nmax; c += 8) my_q[c] = (unsigned short)V3_CAP;
-                    __syncwarp();
-                    for (int c = 0; c < nmax; ++c) {
-                        const unsigned jj = my_q[c];
-                        const float4 e = lds_f4(ent_sa + jj * 16);
-                        const unsigned cm = lds_u32(mask_sa + jj * 4);
-                        const float dx = e.x - fvx, dy = e.y - fvy, dz = e.z - fvz;
-                        const float d2 = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-                        const float qf = e.w * rcp_approx(d2);  // sigma^2/d2; +inf at d2 == 0 -> value 1
-                        // gate on the FMA pipe (the ALU pipe carries the 8 FMNMX and is the busiest unit):
-                        // g = sat(2^100 * (cut_lo - d2)) is exactly 1 for d2 < cut_lo and 0 otherwise (NaN -> 0)
-                        float qv = qf * __saturatef(fmaf(-GATE_SCALE, d2, gate_k));
-                        // d2 in [cut_lo, cut_hi): (d2 - cut_lo) as unsigned bits is < bits(band) only for 0 <= t < band
-                        if (__float_as_uint(d2 - cut_lo) < band_bits) {  // within 4e-6 of the gate: decide like the reference
-                            if (exact_gate(gg, p.coords, s_src[jj], ix, iy, iz)) qv = qf;
-                        }
-#pragma unroll
-                        for (int h = 0; h < 8; ++h)
-                            if (cm & (1u << h)) acc[h] = fmaxf(acc[h], qv);
-                    }
-                    __syncwarp();
-                    cq0 = cq1 = cq2 = cq3 = 0;
-                }
-            }
-        }
-    }
-
-    // ---- epilogue: one transcendental per voxel-channel
-    float v[8];
-    if (touched) {
-#pragma unroll
-        for (int h = 0; h < 8; ++h) v[h] = occ_value(acc[h]);
-    } else {
-#pragma unroll
-        for (int h = 0; h < 8; ++h) v[h] = 0.0f;
-    }
-    if (p.bulk_store) {
-        // TMA path: the tile is staged in shared memory as [x][y][z][channel] (the tile list's storage is dead by now)
-        // and leaves the SM as 64 bulk-async row copies (cp.async.bulk.global.shared::cta, SASS UBLKCP) of up to
-        // 256 contiguous bytes each: full-sector writes, no per-thread store instructions, clipping by row length.
-        __syncthreads();  // every warp is done reading the tile list
-        float4 *const stage = s_ent;
-        const int vt = (vx * TILE + vy) * TILE + vz;
-        stage[vt * 2 + 0] = make_float4(v[0], v[1], v[2], v[3]);
-        stage[vt * 2 + 1] = make_float4(v[4], v[5], v[6], v[7]);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncthreads();
-        if (tid < TILE * TILE) {
-            const int rx = tid >> 3, ry = tid & 7;
-            const int ixr = tx * TILE + rx, iyr = ty * TILE + ry;
-            const int nzr = min(TILE, nz - tz * TILE);
-            if (ixr < nx && iyr < ny) {
-                float *const dst = p.out + (__ldg(&gg->out_offset) + ((long long)ixr * ny + iyr) * nz + tz * TILE) * 8;
-                const unsigned src = (unsigned)__cvta_generic_to_shared(stage + tid * (TILE * 2));
-                asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
-                             :: "l"(dst), "r"(src), "r"(nzr * 32) : "memory");
-            }
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // smem must outlive the copy
-        }
-        return;
-    }
-    if (inside) {
-        const int C = p.C;
-        const long long cs = p.cmajor ? (long long)nx * ny * nz : 1;
-        float *const oo = p.vec_ok ? o : p.out + __ldg(&gg->out_offset) * C +
-                                             (((long long)ix * ny + iy) * nz + iz) * (p.cmajor ? 1 : C);
-        if (p.flags & MKB_OCC_ACCUMULATE) {
-#pragma unroll
-            for (int h = 0; h < 8; ++h)
-                if (h < C) { const float old = oo[h * cs]; v[h] = (acc[h] > 0.0f && v[h] > old) ? v[h] : old; }
-        }
-        if (p.vec_ok) {
-            __stcs(reinterpret_cast<float4 *>(oo), make_float4(v[0], v[1], v[2], v[3]));
-            __stcs(reinterpret_cast<float4 *>(oo) + 1, make_float4(v[4], v[5], v[6], v[7]));
-        } else {
-#pragma unroll
-            for (int h = 0; h < 8; ++h)
-                if (h < C) oo[h * cs] = v[h];
-        }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// K1 warp-per-block path (C <= 8, default): no CTA-level synchronisation at all.
-//   Each WARP owns one 2x4x4 voxel block end to end: it gathers the block's own halo from 4-voxel cells (<= 128
-//   contiguous cell rows), keeps the survivors as records in its private shared-memory list, splits them into the four
-//   2x2x2 quarter lists and runs the lock-step candidate loop.  Compared with the tile kernel above this removes the
-//   three __syncthreads per tile, the intra-CTA load imbalance (a CTA lived as long as its busiest block) and the
-//   stage where all 16 warps re-scanned the whole tile list; empty blocks retire after one row scan.
-//   CTA = 4 warps = 4 z-consecutive blocks, purely a container.
-// ---------------------------------------------------------------------------------------------------------
-constexpr int W_WARPS = 4;
-#ifndef MKB_W_MIN_CTAS
-#define MKB_W_MIN_CTAS 8
-#endif
-constexpr int W_MIN_CTAS = MKB_W_MIN_CTAS;  // resident CTAs per SM the register allocation must allow
-constexpr int W_CELL = 4;    // cell edge of the binning used with this kernel
-constexpr int W_ROWS = 64;    // cell rows per block: (Rx+1)(Ry+1) (cutoff <= 7 voxels -> <= 20)
-constexpr int W_PCAP = 128;   // block candidates per round
-constexpr int W_QCAP = 96;    // sub-block candidates per round
-
-// halo atom count of every 2x4x4 block (one THREAD per block: 32x cheaper than letting each warp find out that
-// its block is empty -- and 70 % of the blocks of a pocket grid are).  block id = ((grid, bx), by, bz) flattened.
-__global__ void occ_block_total_kernel(const GridDev *__restrict__ grids, const unsigned *__restrict__ cell_start,
-                                       const long long *__restrict__ block_base, unsigned *__restrict__ block_total) {
-    const GridDev &g = grids[blockIdx.y];
-    const int nbx = (g.dims[0] + 1) / 2, nby = (g.dims[1] + 3) / 4, nbz = (g.dims[2] + 3) / 4;
+    const int nbx = (g.dims[0] + 1) / 2, nby = (g.dims[1] + 3) / 4, nbz = (g.dims[2] + V_BZ - 1) / V_BZ;
     const int local = blockIdx.x * blockDim.x + threadIdx.x;
     if (local >= nbx * nby * nbz) return;
     const int bzi = local % nbz, bxy = local / nbz, byi = bxy % nby, bxi = bxy / nby;
     const int cutv = g.cutv, cN1 = g.cells[1], cN2 = g.cells[2];
-    const int cx0 = (bxi * 2) / W_CELL, cx1 = min((bxi * 2 + 1 + 2 * cutv) / W_CELL, g.cells[0] - 1);
-    const int cy0 = byi, cy1 = min((byi * 4 + 3 + 2 * cutv) / W_CELL, cN1 - 1);
-    const int cz0 = bzi, cz1 = min((bzi * 4 + 3 + 2 * cutv) / W_CELL, cN2 - 1);
+    const int cx0 = (bxi * 2) / V_CELL, cx1 = min((bxi * 2 + 1 + 2 * cutv) / V_CELL, g.cells[0] - 1);
+    const int cy0 = byi, cy1 = min((byi * 4 + 3 + 2 * cutv) / V_CELL, cN1 - 1);
+    const int cz0 = bzi * (V_BZ / V_CELL), cz1 = min((bzi * V_BZ + V_BZ - 1 + 2 * cutv) / V_CELL, cN2 - 1);
     unsigned total = 0;
     for (int cx = cx0; cx <= cx1; ++cx)
         for (int cy = cy0; cy <= cy1; ++cy) {
@@ -839,317 +494,13 @@ __global__ void occ_block_total_kernel(const GridDev *__restrict__ grids, const 
 // load (its halo count) before it can retire.
 #define WG(field) (UNIFORM ? p.u.field : __ldg(&gg->field))
 template <bool UNIFORM>
-__global__ void __launch_bounds__(W_WARPS * 32, W_MIN_CTAS) occ_fill8w_kernel(const FillParams p, const long long *__restrict__ block_base,
-                                                                     const unsigned *__restrict__ block_total) {
-    __shared__ float4 s_pent[W_WARPS][W_PCAP + 1];    // block candidates: x, y, z in the block frame, sigma^2 (+ sentinel)
-    __shared__ unsigned s_pmask[W_WARPS][W_PCAP + 1];  // channel mask; 0 = several sigmas
-    __shared__ unsigned s_psrc[W_WARPS][W_PCAP];
-    __shared__ unsigned s_rpos[W_WARPS][W_ROWS];
-    __shared__ unsigned s_rbase[W_WARPS][W_ROWS + 1];
-    __shared__ unsigned short s_qidx[W_WARPS][4][W_QCAP];
-
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int bzi = blockIdx.x * W_WARPS + warp, byi = blockIdx.y, bxi = blockIdx.z & ((1 << p.txp_shift) - 1);
-    const int gi = blockIdx.z >> p.txp_shift;
-    const GridDev *gg = p.grids + gi;
-    const int nx = WG(dims[0]), ny = WG(dims[1]), nz = WG(dims[2]);
-    const long long out_offset = UNIFORM ? p.u.out_offset + (long long)gi * p.u_out_stride : __ldg(&gg->out_offset);
-    if (bxi * 2 >= nx || byi * 4 >= ny || bzi * 4 >= nz) return;  // padding of the launch grid / ragged batch
-
-    // ---- empty block (no atom within reach): stream 32 x 32 B of zeros and retire
-    {
-        const int nby = (ny + 3) >> 2, nbz = (nz + 3) >> 2;
-        const long long bb = UNIFORM ? p.u_block_base + (long long)gi * p.u_block_stride : __ldg(block_base + gi);
-        const unsigned tot = __ldg(block_total + bb + ((long long)bxi * nby + byi) * nbz + bzi);
-        if (tot == 0 && p.vec_ok && !(p.flags & MKB_OCC_ACCUMULATE)) {
-            const int ix = bxi * 2 + (lane >> 4), iy = byi * 4 + ((lane >> 2) & 3), iz = bzi * 4 + (lane & 3);
-            if (ix < nx && iy < ny && iz < nz) {
-                float4 *d = reinterpret_cast<float4 *>(p.out + (out_offset + ((long long)ix * ny + iy) * nz + iz) * 8);
-                const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-                __stcs(d, z4);
-                __stcs(d + 1, z4);
-            }
-            return;
-        }
-        if (tot == 0 && p.cmajor && !(p.flags & MKB_OCC_ACCUMULATE)) {  // channel-major: 16-byte z-runs per channel
-            const int ix = bxi * 2 + (lane >> 4), iy = byi * 4 + ((lane >> 2) & 3), iz = bzi * 4 + (lane & 3);
-            if (ix < nx && iy < ny && iz < nz) {
-                const long long cs = (long long)nx * ny * nz;
-                float *d = p.out + out_offset * p.C + ((long long)ix * ny + iy) * nz + iz;
-                for (int h = 0; h < p.C; ++h) __stcs(d + h * cs, 0.f);
-            }
-            return;
-        }
-    }
-
-    // ---- cell rows of this block's halo: shifted voxel range [lo, lo + ext - 1 + 2 cutv] per axis (W_CELL = 4)
-    const int cutv = WG(cutv);
-    const int cN1 = WG(cells[1]), cN2 = WG(cells[2]);
-    const int cx0 = (bxi * 2) / W_CELL, cx1 = min((bxi * 2 + 1 + 2 * cutv) / W_CELL, WG(cells[0]) - 1);
-    const int cy0 = byi, cy1 = min((byi * 4 + 3 + 2 * cutv) / W_CELL, cN1 - 1);
-    const int cz0 = bzi, cz1 = min((bzi * 4 + 3 + 2 * cutv) / W_CELL, cN2 - 1);
-    const int ncy = cy1 - cy0 + 1;
-    const int nrows = (cx1 - cx0 + 1) * ncy;  // <= W_ROWS checked on the host
-    unsigned *const rpos = s_rpos[warp], *const rbase = s_rbase[warp];
-    const long long cell_base = UNIFORM ? p.u.cell_base + (long long)gi * p.u_cell_stride : __ldg(&gg->cell_base);
-    const float inv_ncy = 1.0f / (float)ncy;
-    unsigned carry = 0;
-    for (int r0 = 0; r0 < nrows; r0 += 32) {  // row lengths + inclusive scan, 32 rows per step
-        const int r = r0 + lane;
-        unsigned v = 0;
-        if (r < nrows) {
-            const int rx = (int)(((float)r + 0.5f) * inv_ncy), ry = r - rx * ncy;  // exact for small r
-            const long long cb = cell_base + ((long long)(cx0 + rx) * cN1 + (cy0 + ry)) * cN2;
-            const unsigned a = __ldg(p.cell_start + cb + cz0);
-            v = __ldg(p.cell_start + cb + cz1 + 1) - a;
-            rpos[r] = a;
-        }
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned t = __shfl_up_sync(0xffffffffu, v, o);
-            if (lane >= o) v += t;
-        }
-        if (r < nrows) rbase[r + 1] = v + carry;
-        carry += __shfl_sync(0xffffffffu, v, 31);
-    }
-    const unsigned total = carry;
-
-    // lane -> voxel of the block (block frame: origin at the block centre)
-    const int q = lane >> 3, sub = lane & 7;
-    const int lx = sub >> 2, ly = (q >> 1) * 2 + ((sub >> 1) & 1), lz = (q & 1) * 2 + (sub & 1);
-    const int ix = bxi * 2 + lx, iy = byi * 4 + ly, iz = bzi * 4 + lz;
-    const bool inside = ix < nx && iy < ny && iz < nz;
-
-    float acc[8];
-#pragma unroll
-    for (int h = 0; h < 8; ++h) acc[h] = 0.0f;
-    bool touched = false;
-
-    if (total != 0) {
-        if (lane == 0) {
-            rbase[0] = 0;
-            s_pent[warp][W_PCAP] = make_float4(1e18f, 1e18f, 1e18f, 0.0f);  // sentinel: never inside the gate
-            s_pmask[warp][W_PCAP] = 1u;
-        }
-        __syncwarp();
-        const float cut_lo = WG(cut2v_lo), cut_hi = WG(cut2v_hi);
-        const float gate_k = GATE_SCALE * cut_lo;
-        const unsigned band_bits = __float_as_uint(cut_hi - cut_lo);
-        const float fvx = (float)lx - 0.5f, fvy = (float)ly - 1.5f, fvz = (float)lz - 1.5f;
-        // cell origin -> block-centre frame: (c * cell - cutv) - (block corner + half extent)
-        const int sx = bxi * 2 + cutv, sy = byi * 4 + cutv, sz = bzi * 4 + cutv;
-        float4 *const pent = s_pent[warp];
-        unsigned *const pmask = s_pmask[warp], *const psrc = s_psrc[warp];
-        unsigned short *const my_q = s_qidx[warp][q];
-        unsigned ent_sa, mask_sa;
-        asm volatile("{ .reg .u64 t; cvta.to.shared.u64 t, %1; cvt.u32.u64 %0, t; }" : "=r"(ent_sa) : "l"(pent));
-        asm volatile("{ .reg .u64 t; cvta.to.shared.u64 t, %1; cvt.u32.u64 %0, t; }" : "=r"(mask_sa) : "l"(pmask));
-
-        int np = 0;
-        int row = 0;  // row of this lane's current atom: k only grows, so the row pointer only advances
-        for (unsigned k0 = 0; k0 < total; k0 += 32) {
-            // ---- gather 32 atoms of the concatenated cell rows, keep those within reach of the block
-            {
-                const unsigned k = min(k0 + lane, total - 1);
-                while (rbase[row + 1] <= k) ++row;  // rbase[nrows] == total > k: terminates
-                const unsigned i = rpos[row] + (k - rbase[row]);
-                float4 e = __ldg(p.rec_pos + i);
-                const uint4 tg = __ldg(p.rec_tag + i);
-                e.x += (float)((int)(tg.z & 1023u) * W_CELL - sx) - 0.5f;  // exact: small integers and halves
-                e.y += (float)((int)((tg.z >> 10) & 1023u) * W_CELL - sy) - 1.5f;
-                e.z += (float)((int)(tg.z >> 20) * W_CELL - sz) - 1.5f;
-                const float ddx = fmaxf(fabsf(e.x) - 0.5f, 0.f);
-                const float ddy = fmaxf(fabsf(e.y) - 1.5f, 0.f);
-                const float ddz = fmaxf(fabsf(e.z) - 1.5f, 0.f);
-                const bool pass = (k0 + lane < total) & (tg.x != 0) & (fmaf(ddz, ddz, fmaf(ddy, ddy, ddx * ddx)) <= cut_hi);
-                const unsigned bal = __ballot_sync(0xffffffffu, pass);
-                if (pass) {
-                    const int slot = np + __popc(bal & ((1u << lane) - 1u));
-                    pent[slot] = e;
-                    pmask[slot] = (tg.y & 0x80000000u) ? 0u : tg.x;
-                    psrc[slot] = tg.y & 0x7fffffffu;
-                }
-                np += __popc(bal);
-            }
-            if (np <= W_PCAP - 32 && k0 + 32 < total) continue;
-            if (np == 0) continue;
-            touched = true;
-            __syncwarp();
-            // ---- block list -> four 2x2x2 sub-block lists, evaluated in lock-step
-            int cq0 = 0, cq1 = 0, cq2 = 0, cq3 = 0;
-            for (int j0 = 0; j0 < np; j0 += 32) {
-                const int j = j0 + lane;
-                const bool live = j < np;
-                const unsigned idx = min(j, np - 1);
-                bool h0, h1, h2, h3, multi;
-                {
-                    const float4 e = lds_f4(ent_sa + idx * 16);
-                    const float ddx = fmaxf(fabsf(e.x) - 0.5f, 0.f);
-                    const float y0 = fmaxf(fabsf(e.y + 1.f) - 0.5f, 0.f), y1 = fmaxf(fabsf(e.y - 1.f) - 0.5f, 0.f);
-                    const float z0 = fmaxf(fabsf(e.z + 1.f) - 0.5f, 0.f), z1 = fmaxf(fabsf(e.z - 1.f) - 0.5f, 0.f);
-                    const float xx = ddx * ddx;
-                    const float a0 = fmaf(y0, y0, xx), a1 = fmaf(y1, y1, xx);
-                    multi = live & (lds_u32(mask_sa + idx * 4) == 0);
-                    const bool ok = live & !multi;
-                    h0 = ok & (fmaf(z0, z0, a0) <= cut_hi);  // q = qy*2 + qz
-                    h1 = ok & (fmaf(z1, z1, a0) <= cut_hi);
-                    h2 = ok & (fmaf(z0, z0, a1) <= cut_hi);
-                    h3 = ok & (fmaf(z1, z1, a1) <= cut_hi);
-                }
-                // atoms carrying several distinct sigmas (user float channels): whole-warp per-channel path
-                for (unsigned bm = __ballot_sync(0xffffffffu, multi); bm; bm &= bm - 1) {
-                    const int jj = j0 + __ffs(bm) - 1;
-                    const float4 e = pent[jj];
-                    const float dx = e.x - fvx, dy = e.y - fvy, dz = e.z - fvz;
-                    const float d2 = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-                    bool in = d2 < cut_lo;
-                    if (!in && d2 < cut_hi) in = exact_gate(gg, p.coords, psrc[jj], ix, iy, iz);
-                    const float rr = in ? rcp_approx(d2) : 0.0f;
-                    const double *sg = p.sigmas + (long long)psrc[jj] * p.C;
-                    const double ivs = WG(inv_vs);
-#pragma unroll
-                    for (int h = 0; h < 8; ++h) {
-                        if (h < p.C) {
-                            const double sv = sg[h] * ivs;
-                            const float sq = (sv == 0.0 || sv != sv) ? 0.0f : fmaxf((float)(sv * sv), FLT_MIN);
-                            acc[h] = fmaxf(acc[h], sq * rr);  // 0*inf = NaN is dropped by fmaxf
-                        }
-                    }
-                }
-                const unsigned lt = (1u << lane) - 1u;
-                const unsigned b0 = __ballot_sync(0xffffffffu, h0), b1 = __ballot_sync(0xffffffffu, h1);
-                const unsigned b2 = __ballot_sync(0xffffffffu, h2), b3 = __ballot_sync(0xffffffffu, h3);
-                unsigned short *const wq = s_qidx[warp][0];
-                if (h0) wq[0 * W_QCAP + cq0 + __popc(b0 & lt)] = (unsigned short)idx;
-                if (h1) wq[1 * W_QCAP + cq1 + __popc(b1 & lt)] = (unsigned short)idx;
-                if (h2) wq[2 * W_QCAP + cq2 + __popc(b2 & lt)] = (unsigned short)idx;
-                if (h3) wq[3 * W_QCAP + cq3 + __popc(b3 & lt)] = (unsigned short)idx;
-                cq0 += __popc(b0); cq1 += __popc(b1); cq2 += __popc(b2); cq3 += __popc(b3);
-                const int nmax = max(max(cq0, cq1), max(cq2, cq3));
-                if (j0 + 32 < np && nmax <= W_QCAP - 32) continue;
-                // pad the shorter quarters with the sentinel, then run all four lists in lock-step
-                const int mine = (q == 0) ? cq0 : (q == 1) ? cq1 : (q == 2) ? cq2 : cq3;
-                for (int c = mine + sub; c < nmax; c += 8) my_q[c] = (unsigned short)W_PCAP;
-                __syncwarp();
-                for (int c = 0; c < nmax; ++c) {
-                    const unsigned jj = my_q[c];
-                    const float4 e = lds_f4(ent_sa + jj * 16);
-                    const unsigned cm = lds_u32(mask_sa + jj * 4);
-                    const float dx = e.x - fvx, dy = e.y - fvy, dz = e.z - fvz;
-                    const float d2 = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-                    const float qf = e.w * rcp_approx(d2);  // sigma^2/d2; +inf at d2 == 0 -> value 1
-                    float qv = qf * __saturatef(fmaf(-GATE_SCALE, d2, gate_k));  // exact 0/1 gate on the FMA pipe
-                    if (__float_as_uint(d2 - cut_lo) < band_bits) {  // within 4e-6 of the gate: decide like the reference
-                        if (exact_gate(gg, p.coords, psrc[jj], ix, iy, iz)) qv = qf;
-                    }
-#pragma unroll
-                    for (int h = 0; h < 8; ++h)
-                        if (cm & (1u << h)) acc[h] = fmaxf(acc[h], qv);
-                }
-                __syncwarp();
-                cq0 = cq1 = cq2 = cq3 = 0;
-            }
-            np = 0;
-            __syncwarp();
-        }
-    }
-
-    // ---- epilogue: one transcendental per voxel-channel, 32-byte streaming stores (4 lanes = one 128-byte line)
-    if (inside) {
-        const int C = p.C;
-        float v[8];
-        if (touched) {
-#pragma unroll
-            for (int h = 0; h < 8; ++h) v[h] = occ_value(acc[h]);
-        } else {
-#pragma unroll
-            for (int h = 0; h < 8; ++h) v[h] = 0.0f;
-        }
-        const long long cs = p.cmajor ? (long long)nx * ny * nz : 1;
-        float *const oo = p.out + out_offset * C + (((long long)ix * ny + iy) * nz + iz) * (p.cmajor ? 1 : C);
-        if (p.flags & MKB_OCC_ACCUMULATE) {
-#pragma unroll
-            for (int h = 0; h < 8; ++h)
-                if (h < C) { const float old = oo[h * cs]; v[h] = (acc[h] > 0.0f && v[h] > old) ? v[h] : old; }
-        }
-        if (p.vec_ok) {
-            __stcs(reinterpret_cast<float4 *>(oo), make_float4(v[0], v[1], v[2], v[3]));
-            __stcs(reinterpret_cast<float4 *>(oo) + 1, make_float4(v[4], v[5], v[6], v[7]));
-        } else if (p.cmajor) {
-#pragma unroll
-            for (int h = 0; h < 8; ++h)
-                if (h < C) __stcs(oo + h * cs, v[h]);
-        } else {
-#pragma unroll
-            for (int h = 0; h < 8; ++h)
-                if (h < C) oo[h] = v[h];
-        }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// K1 v6 (default for C <= 8, cutoff <= 7 voxels): one warp = one 2x4x8 block, TWO voxels per lane.
-//   The block is eight 2x2x2 sub-blocks (sy in 0..1, sz in 0..3), four lanes each; a lane owns the x-pair of voxels
-//   (0, y, z) and (1, y, z).  Against the 2x4x4 kernel above:
-//     * one halo gather (cell rows are contiguous along z, so doubling the block along z adds ~20 % scanned atoms, not
-//       100 %), one row set-up, one prologue per 64 voxels instead of per 32;
-//     * a candidate is loaded once for two voxels that share dy, dz and the channel mask: 39 instructions per candidate
-//       for two pairs instead of 30 for one, while each 2x2x2 sub-block keeps its own list (same 47 % hit rate);
-//     * two independent dependency chains per lane (ILP) stand in for the halved number of resident warps.
-// ---------------------------------------------------------------------------------------------------------
-constexpr int V_BZ = 8;       // block extent along z
-#ifndef MKB_V_PCAP
-#define MKB_V_PCAP 192  // capacity sweep (ms per 256 pockets): 128/96 1.864, 160/96 1.858, 224/96 1.841, 192/128 1.814, 224/128 1.825, 256/128 1.850
-#endif
-#ifndef MKB_V_QCAP
-#define MKB_V_QCAP 128
-#endif
-constexpr int V_PCAP = MKB_V_PCAP;   // block candidates per round
-constexpr int V_QCAP = MKB_V_QCAP;   // sub-block candidates per round
-constexpr int V_QSTRIDE = V_QCAP + 2;  // + one sentinel slot for the software-pipelined loop
-#ifndef MKB_V_UNROLL2
-#define MKB_V_UNROLL2 0  // two candidates per trip (spills at 72 registers)
-#endif
-#ifndef MKB_V_WARPS
-#define MKB_V_WARPS 1    // warps (= blocks) per CTA. A CTA holds its registers until its slowest warp retires
-#endif
-constexpr int V_WARPS = MKB_V_WARPS;
-#ifndef MKB_V_ZPER
-#define MKB_V_ZPER 1     // consecutive z blocks walked by one warp (longer-lived CTAs balance worse)
-#endif
-constexpr int V_ZPER = MKB_V_ZPER;
-#ifndef MKB_V_MIN_CTAS
-#define MKB_V_MIN_CTAS 7  // 72 registers; at 8 CTAs (64 registers) the kernel spills
-#endif
-
-__global__ void occ_block_total_v_kernel(const GridDev *__restrict__ grids, const unsigned *__restrict__ cell_start,
-                                         const long long *__restrict__ block_base, unsigned *__restrict__ block_total) {
-    const GridDev &g = grids[blockIdx.y];
-    const int nbx = (g.dims[0] + 1) / 2, nby = (g.dims[1] + 3) / 4, nbz = (g.dims[2] + V_BZ - 1) / V_BZ;
-    const int local = blockIdx.x * blockDim.x + threadIdx.x;
-    if (local >= nbx * nby * nbz) return;
-    const int bzi = local % nbz, bxy = local / nbz, byi = bxy % nby, bxi = bxy / nby;
-    const int cutv = g.cutv, cN1 = g.cells[1], cN2 = g.cells[2];
-    const int cx0 = (bxi * 2) / W_CELL, cx1 = min((bxi * 2 + 1 + 2 * cutv) / W_CELL, g.cells[0] - 1);
-    const int cy0 = byi, cy1 = min((byi * 4 + 3 + 2 * cutv) / W_CELL, cN1 - 1);
-    const int cz0 = bzi * (V_BZ / W_CELL), cz1 = min((bzi * V_BZ + V_BZ - 1 + 2 * cutv) / W_CELL, cN2 - 1);
-    unsigned total = 0;
-    for (int cx = cx0; cx <= cx1; ++cx)
-        for (int cy = cy0; cy <= cy1; ++cy) {
-            const long long cb = g.cell_base + ((long long)cx * cN1 + cy) * cN2;
-            total += cell_start[cb + cz1 + 1] - cell_start[cb + cz0];
-        }
-    block_total[block_base[blockIdx.y] + local] = total;
-}
-
-template <bool UNIFORM>
-__global__ void __launch_bounds__(V_WARPS * 32, MKB_V_MIN_CTAS * 4 / V_WARPS)
+__global__ void __launch_bounds__(V_WARPS * 32, V_MIN_CTAS * 4 / V_WARPS)
 occ_fill8v_kernel(const FillParams p, const long long *__restrict__ block_base, const unsigned *__restrict__ block_total) {
     __shared__ float4 s_pent[V_WARPS][V_PCAP + 1];    // block candidates: x, y, z in the block frame, sigma^2 (+ sentinel)
     __shared__ unsigned s_pmask[V_WARPS][V_PCAP + 1];  // channel mask; 0 = several sigmas
     __shared__ unsigned s_psrc[V_WARPS][V_PCAP];
-    __shared__ unsigned s_rpos[V_WARPS][W_ROWS];
-    __shared__ unsigned s_rbase[V_WARPS][W_ROWS + 1];
+    __shared__ unsigned s_rpos[V_WARPS][V_ROWS];
+    __shared__ unsigned s_rbase[V_WARPS][V_ROWS + 1];
     __shared__ unsigned short s_qidx[V_WARPS][8][V_QSTRIDE];
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1162,11 +513,8 @@ occ_fill8v_kernel(const FillParams p, const long long *__restrict__ block_base, 
     const int C = p.C;
     const long long cs = p.cmajor ? (long long)nx * ny * nz : 1;  // channel stride; voxel stride is C or 1
     const int vstride = p.cmajor ? 1 : C;
-    // a warp walks V_ZPER consecutive blocks of its (x, y) column: fewer, longer-lived CTAs (the 70 % empty blocks no
-    // longer cost a CTA launch each) while the work per CTA stays small against the number of CTAs
-    for (int zi = 0; zi < V_ZPER; ++zi) {
-    const int bzi = (blockIdx.x * V_ZPER + zi) * V_WARPS + warp;
-    if (bzi * V_BZ >= nz) break;
+    const int bzi = blockIdx.x * V_WARPS + warp;
+    if (bzi * V_BZ >= nz) return;
 
     // ---- empty block (no atom within reach): stream 64 x 32 B of zeros and retire
     {
@@ -1191,18 +539,18 @@ occ_fill8v_kernel(const FillParams p, const long long *__restrict__ block_base, 
                     }
                 }
             }
-            continue;
+            return;
         }
     }
 
-    // ---- cell rows of this block's halo (W_CELL = 4): rows run along z
+    // ---- cell rows of this block's halo (V_CELL = 4): rows run along z
     const int cutv = WG(cutv);
     const int cN1 = WG(cells[1]), cN2 = WG(cells[2]);
-    const int cx0 = (bxi * 2) / W_CELL, cx1 = min((bxi * 2 + 1 + 2 * cutv) / W_CELL, WG(cells[0]) - 1);
-    const int cy0 = byi, cy1 = min((byi * 4 + 3 + 2 * cutv) / W_CELL, cN1 - 1);
-    const int cz0 = bzi * (V_BZ / W_CELL), cz1 = min((bzi * V_BZ + V_BZ - 1 + 2 * cutv) / W_CELL, cN2 - 1);
+    const int cx0 = (bxi * 2) / V_CELL, cx1 = min((bxi * 2 + 1 + 2 * cutv) / V_CELL, WG(cells[0]) - 1);
+    const int cy0 = byi, cy1 = min((byi * 4 + 3 + 2 * cutv) / V_CELL, cN1 - 1);
+    const int cz0 = bzi * (V_BZ / V_CELL), cz1 = min((bzi * V_BZ + V_BZ - 1 + 2 * cutv) / V_CELL, cN2 - 1);
     const int ncy = cy1 - cy0 + 1;
-    const int nrows = (cx1 - cx0 + 1) * ncy;  // <= W_ROWS checked on the host
+    const int nrows = (cx1 - cx0 + 1) * ncy;  // <= V_ROWS checked on the host
     unsigned *const rpos = s_rpos[warp], *const rbase = s_rbase[warp];
     const long long cell_base = UNIFORM ? p.u.cell_base + (long long)gi * p.u_cell_stride : __ldg(&gg->cell_base);
     const float inv_ncy = 1.0f / (float)ncy;
@@ -1219,9 +567,9 @@ occ_fill8v_kernel(const FillParams p, const long long *__restrict__ block_base, 
             rpos[r] = a;
             // corner rows: the cell column [c*4 - cutv, c*4 + 4 - cutv) is further than the cutoff from the block's
             // x/y extent -> none of its atoms can pass the cull below, skip the row
-            const int lox = (cx0 + rx) * W_CELL - cutv, loy = (cy0 + ry) * W_CELL - cutv;
-            const int gx = max(max(lox - (bxi * 2 + 1), bxi * 2 - (lox + W_CELL)), 0);
-            const int gy = max(max(loy - (byi * 4 + 3), byi * 4 - (loy + W_CELL)), 0);
+            const int lox = (cx0 + rx) * V_CELL - cutv, loy = (cy0 + ry) * V_CELL - cutv;
+            const int gx = max(max(lox - (bxi * 2 + 1), bxi * 2 - (lox + V_CELL)), 0);
+            const int gy = max(max(loy - (byi * 4 + 3), byi * 4 - (loy + V_CELL)), 0);
             if ((float)(gx * gx + gy * gy) > cut_hi_row) v = 0;
         }
 #pragma unroll
@@ -1276,9 +624,9 @@ occ_fill8v_kernel(const FillParams p, const long long *__restrict__ block_base, 
                 const unsigned i = rpos[row] + (k - rbase[row]);
                 float4 e = __ldg(p.rec_pos + i);
                 const uint4 tg = __ldg(p.rec_tag + i);
-                e.x += (float)((int)(tg.z & 1023u) * W_CELL - sx) - 0.5f;  // exact: small integers and halves
-                e.y += (float)((int)((tg.z >> 10) & 1023u) * W_CELL - sy) - 1.5f;
-                e.z += (float)((int)(tg.z >> 20) * W_CELL - sz) - 3.5f;
+                e.x += (float)((int)(tg.z & 1023u) * V_CELL - sx) - 0.5f;  // exact: small integers and halves
+                e.y += (float)((int)((tg.z >> 10) & 1023u) * V_CELL - sy) - 1.5f;
+                e.z += (float)((int)(tg.z >> 20) * V_CELL - sz) - 3.5f;
                 const float ddx = fmaxf(fabsf(e.x) - 0.5f, 0.f);
                 const float ddy = fmaxf(fabsf(e.y) - 1.5f, 0.f);
                 const float ddz = fmaxf(fabsf(e.z) - 3.5f, 0.f);
@@ -1386,15 +734,7 @@ occ_fill8v_kernel(const FillParams p, const long long *__restrict__ block_base, 
                     for (int h = 0; h < 8; ++h)
                         if (cm & (1u << h)) { acc0[h] = fmaxf(acc0[h], qv0); acc1[h] = fmaxf(acc1[h], qv1); }
                 };
-#if MKB_V_UNROLL2
-                // two candidates per trip; slot nmax holds a sentinel, so an odd list simply evaluates it once
-                for (unsigned qa = q_sa, qe = q_sa + 2 * nmax; qa < qe; qa += 4) {
-                    candidate(qa);
-                    candidate(qa + 2);
-                }
-#else
                 for (unsigned qa = q_sa, qe = q_sa + 2 * nmax; qa < qe; qa += 2) candidate(qa);
-#endif
                 __syncwarp();
 #pragma unroll
                 for (int u = 0; u < 8; ++u) cq[u] = 0;
@@ -1444,8 +784,7 @@ occ_fill8v_kernel(const FillParams p, const long long *__restrict__ block_base, 
             }
         }
     }
-    __syncwarp();  // the lists are reused by the next block
-    }
+    __syncwarp();  // no data hazard left; without it ptxas schedules the measured kernel differently
 }
 #undef WG
 
@@ -1607,6 +946,28 @@ static int scan_u32(mkb_ctx *h, cudaStream_t st, unsigned *in, unsigned *out, lo
 
 using namespace mkb;
 
+// The fill kernel of a call, chosen once for the batch from its finest grid (the largest cutoff in voxels, cv):
+//   runs     occ_fill_runs_kernel: 8 channels, no accumulate, 16-byte aligned output, cv <= 40 (voxelsize >= 0.125 A,
+//            the range it is tested and measured on); the caller still drops it when the batch exceeds its index limits;
+//   warp     otherwise, with <= 8 channels, occ_fill8v_kernel while a block's halo fits in V_ROWS cell rows (cv <= 14);
+//   generic  otherwise occ_fill_kernel<CP>.
+// MKB_OCC_V6 and MKB_OCC_GENERIC put the same input through a fallback, so tests can compare the kernels.
+struct FillChoice {
+    bool runs, warp;
+};
+static FillChoice choose_fill_kernel(int C, uint32_t flags, const float *out, const mkb_grid_desc *grids, int B) {
+    int cv = 0;
+    for (int b = 0; b < B; ++b) {
+        if (!(grids[b].voxelsize > 0.0)) break;  // reported by the caller
+        cv = std::max(cv, (int)std::ceil(CUTOFF_A / grids[b].voxelsize));
+    }
+    const bool generic = getenv("MKB_OCC_GENERIC") != nullptr;
+    FillChoice f;
+    f.runs = C == 8 && !(flags & MKB_OCC_ACCUMULATE) && (uintptr_t)out % 16 == 0 && cv <= 40 && !generic && !getenv("MKB_OCC_V6");
+    f.warp = C <= 8 && ((1 + 2 * cv) / V_CELL + 1) * ((3 + 2 * cv) / V_CELL + 1) <= V_ROWS && !generic;
+    return f;
+}
+
 static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *coords, const double *sigmas,
                                      const double *radii, const uint32_t *chanmask, int64_t n_atoms, int32_t C,
                                      const mkb_grid_desc *grids, int32_t B, float *out, uint32_t flags,
@@ -1622,22 +983,8 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
     if (n_atoms > 0 && (!coords || (!sigmas && (!radii || !chanmask))))
         return fail(h, MKB_ERR_BAD_ARG, "null coords/sigmas");
 
-    // kernel variant: 0 = warp-per-block (C <= 8, default), 1 = tile kernel with quarter lists (MKB_OCC_TILE=1),
-    // 2 = generic tile kernel (9..32 channels, very small voxels, or MKB_OCC_GENERIC=1).  It fixes the cell size.
-    int variant = (C <= 8) ? 0 : 2;
-    if (variant == 0 && getenv("MKB_OCC_TILE")) variant = 1;
-    const bool force_warp = getenv("MKB_OCC_WARP") != nullptr;
-    if (getenv("MKB_OCC_GENERIC")) variant = 2;
-    for (int b = 0; b < B && variant != 2; ++b) {
-        if (!(grids[b].voxelsize > 0.0)) break;  // reported below
-        const int cv = (int)std::ceil(CUTOFF_A / grids[b].voxelsize);
-        // very fine grids: the halo of a block spans more cell rows than a warp keeps (cutoff > 11 voxels) -> tile kernel.
-        // (MKB_OCC_WARP32=1 restores the older rule -- the tile kernel for every cutoff > 7 voxels -- and the older kernel.)
-        const bool old_rule = getenv("MKB_OCC_WARP32") != nullptr && cv > 7 && !force_warp;
-        if (variant == 0 && (old_rule || ((1 + 2 * cv) / 4 + 1) * ((3 + 2 * cv) / 4 + 1) > W_ROWS)) variant = 1;
-        if (variant == 1 && ((TILE - 1 + 2 * cv) / TILE + 1) * ((TILE - 1 + 2 * cv) / TILE + 1) > 128) variant = 2;
-    }
-    const int cellsz = (variant == 0) ? W_CELL : TILE;
+    const FillChoice fill = choose_fill_kernel(C, flags, out, grids, B);
+    const int cellsz = fill.warp ? V_CELL : TILE;
 
     std::vector<GridDev> gd((size_t)B);
     long long items = 0, tiles = 0, cells = 0, voxels = 0;
@@ -1690,11 +1037,8 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
     if (cells >= (1ll << 31) - 2 || items >= (1ll << 31))
         return fail(h, MKB_ERR_BAD_ARG, "batch too large (%lld cells, %lld atom items): split it", cells, items);
 
-    // ---- default for 8 channels: per-block candidate lists + persistent mask-run kernel with TMA stores (occ_runs.cuh).
-    // MKB_OCC_V6=1 or any of the older selectors keeps the v6 warp kernel (A/B runs,
-    // tests/test_occupancy_gpu.py::test_alternative_kernel_paths_agree); accumulate calls stay on v6 as well.
-    bool use_runs = (variant == 0 || (variant == 1 && !getenv("MKB_OCC_TILE"))) && C == 8 && !(flags & MKB_OCC_ACCUMULATE) && ((uintptr_t)out % 16 == 0) &&
-                    !getenv("MKB_OCC_V6") && !force_warp && !getenv("MKB_OCC_WARP32");
+    // ---- default for 8 channels: per-block candidate lists + persistent mask-run kernel with TMA stores (occ_runs.cuh)
+    bool use_runs = fill.runs;
     std::vector<long long> ibase;
     long long run_blocks = 0, run_items = 0, ent_bound = 0;
     int list_table = 1;  // the list passes count per CTA in shared memory (occ_runs.cuh): off for fine voxels
@@ -1709,7 +1053,6 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
                 it4 += (long long)((gd[b].dims[0] + 3) / 4) * ((gd[b].dims[1] + 3) / 4) * (((gd[b].dims[2] + R_BZ - 1) / R_BZ + R_ZC - 1) / R_ZC);
             const long long warps = (long long)h->sm_count * MKB_R_MIN_CTAS * R_WARPS;
             run_zc = it4 >= 8 * warps ? R_ZC : (it4 >= 3 * warps ? 2 : 1);
-            if (getenv("MKB_OCC_ZC")) run_zc = std::max(1, std::min(R_ZC, atoi(getenv("MKB_OCC_ZC"))));
         }
         for (int b = 0; b < B; ++b) {
             const GridDev &g = gd[b];
@@ -1923,24 +1266,15 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
     fp.cmajor = (flags & MKB_OCC_LAYOUT_CXYZ) ? 1 : 0;
     fp.vec_ok = (C == 8 && ((uintptr_t)out % 16 == 0) && !fp.cmajor) ? 1 : 0;
     fp.txp_shift = 0;
-    // opt-in (MKB_OCC_BULK_STORE=1): slower in this non-persistent kernel because the CTA has to wait for
-    // the asynchronous smem read before it may retire; kept for the persistent variant (DESIGN.md section 6)
-    fp.bulk_store = (fp.vec_ok && !(flags & MKB_OCC_ACCUMULATE) && getenv("MKB_OCC_BULK_STORE")) ? 1 : 0;
 
     if (h->timing) MKB_CUDA(h, cudaEventRecord(h->ev[1], st));
-    const bool fast8 = (variant == 1);
-    unsigned *tile_total = nullptr;
-    if (fast8 && (rc = scratch_get(h, S_TILE_TOTAL, (size_t)tiles, &tile_total))) return rc;
-    if (variant == 0) {
-        // per-block halo counts (thread per block), then the warp-per-block kernel:
-        // grid = (z-blocks / 4, y-blocks, grid << sh | x-block)
-        // block = 2x4xBZ voxels per warp: BZ = 8 with two voxels per lane (default), 4 with MKB_OCC_WARP32=1 (A/B)
-        const bool v64 = getenv("MKB_OCC_WARP32") == nullptr;
-        const int BZ = v64 ? V_BZ : 4;
+    if (fill.warp) {
+        // per-block halo counts (thread per block), then the warp-per-block kernel on 2x4x8-voxel blocks:
+        // grid = (z-blocks, y-blocks, grid << sh | x-block)
         std::vector<long long> bbase((size_t)B + 1, 0);
         long long maxblk = 0;
         for (int b = 0; b < B; ++b) {
-            const long long nbk = (long long)((gd[b].dims[0] + 1) / 2) * ((gd[b].dims[1] + 3) / 4) * ((gd[b].dims[2] + BZ - 1) / BZ);
+            const long long nbk = (long long)((gd[b].dims[0] + 1) / 2) * ((gd[b].dims[1] + 3) / 4) * ((gd[b].dims[2] + V_BZ - 1) / V_BZ);
             bbase[b + 1] = bbase[b] + nbk;
             maxblk = std::max(maxblk, nbk);
         }
@@ -1951,8 +1285,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         MKB_CUDA(h, cudaMemcpyAsync(d_bbase, bbase.data(), sizeof(long long) * ((size_t)B + 1), cudaMemcpyHostToDevice, st));
         for (int c0 = 0; c0 < B; c0 += 65535) {
             const int cn = std::min(65535, B - c0);
-            if (v64) occ_block_total_v_kernel<<<dim3((unsigned)cdiv(maxblk, 256), (unsigned)cn), 256, 0, st>>>(d_grids + c0, cell_start, d_bbase + c0, d_btotal);
-            else occ_block_total_kernel<<<dim3((unsigned)cdiv(maxblk, 256), (unsigned)cn), 256, 0, st>>>(d_grids + c0, cell_start, d_bbase + c0, d_btotal);
+            occ_block_total_v_kernel<<<dim3((unsigned)cdiv(maxblk, 256), (unsigned)cn), 256, 0, st>>>(d_grids + c0, cell_start, d_bbase + c0, d_btotal);
             MKB_LAUNCHED(h);
         }
         int b0 = 0;
@@ -1965,7 +1298,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
                 if (((long long)(nb + 1) << s2) > 65535) break;
                 mx = ax; sh = s2; ++nb;
                 my = std::max(my, (gd[b].dims[1] + 3) / 4);
-                mz = std::max(mz, (gd[b].dims[2] + BZ - 1) / BZ);
+                mz = std::max(mz, (gd[b].dims[2] + V_BZ - 1) / V_BZ);
             }
             if (nb == 0 || my > 65535) return fail(h, MKB_ERR_BAD_ARG, "grid %d too large for one launch", b0);
             FillParams fq = fp;
@@ -1991,46 +1324,23 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
                 const float band = g0.cut2v_hi - g0.cut2v_lo;
                 memcpy(&fq.u_band_bits, &band, sizeof(float));
             }
-            const dim3 wgrid((unsigned)cdiv(mz, W_WARPS), (unsigned)my, (unsigned)(nb << sh));
-            h->last_kernel = v64 ? "occ_fill8v_kernel" : "occ_fill8w_kernel";
-            if (v64) {
-                const dim3 vgrid((unsigned)cdiv(mz, V_WARPS * V_ZPER), (unsigned)my, (unsigned)(nb << sh));
-                if (uni) occ_fill8v_kernel<true><<<vgrid, V_WARPS * 32, 0, st>>>(fq, d_bbase + b0, d_btotal);
-                else occ_fill8v_kernel<false><<<vgrid, V_WARPS * 32, 0, st>>>(fq, d_bbase + b0, d_btotal);
-            } else if (uni) occ_fill8w_kernel<true><<<wgrid, W_WARPS * 32, 0, st>>>(fq, d_bbase + b0, d_btotal);
-            else occ_fill8w_kernel<false><<<wgrid, W_WARPS * 32, 0, st>>>(fq, d_bbase + b0, d_btotal);
+            h->last_kernel = "occ_fill8v_kernel";
+            const dim3 vgrid((unsigned)cdiv(mz, V_WARPS), (unsigned)my, (unsigned)(nb << sh));
+            if (uni) occ_fill8v_kernel<true><<<vgrid, V_WARPS * 32, 0, st>>>(fq, d_bbase + b0, d_btotal);
+            else occ_fill8v_kernel<false><<<vgrid, V_WARPS * 32, 0, st>>>(fq, d_bbase + b0, d_btotal);
             MKB_LAUNCHED(h);
             b0 += nb;
         }
     }
-    for (int b0 = 0; b0 < B && variant != 0; b0 += 65535) {  // tile kernels: blockIdx.y = grid of the batch
+    for (int b0 = 0; b0 < B && !fill.warp; b0 += 65535) {  // tile kernel: blockIdx.y = grid of the batch
         const int nb = std::min(65535, B - b0);
         fp.grids = d_grids + b0;
         fp.B = nb;
         long long mt = 0;
         for (int b = b0; b < b0 + nb; ++b) mt = std::max<long long>(mt, (long long)gd[b].tiles[0] * gd[b].tiles[1] * gd[b].tiles[2]);
         const dim3 grid((unsigned)mt, (unsigned)nb);
-        h->last_kernel = fast8 ? "occ_fill8_kernel" : "occ_fill_kernel";
-        if (fast8) {
-            occ_tile_total_kernel<<<dim3((unsigned)cdiv(mt, 128), (unsigned)nb), 128, 0, st>>>(fp.grids, cell_start, tile_total);
-            MKB_LAUNCHED(h);
-            int mx = 1, my = 1, mz = 1;
-            for (int b = b0; b < b0 + nb; ++b) {
-                mx = std::max(mx, gd[b].tiles[0]); my = std::max(my, gd[b].tiles[1]); mz = std::max(mz, gd[b].tiles[2]);
-            }
-            int sh = 0;
-            while ((1 << sh) < mx) ++sh;
-            fp.txp_shift = sh;
-            const int per_launch = std::max(1, 65535 >> sh);  // gridDim.z <= 65535
-            if (my > 65535) return fail(h, MKB_ERR_BAD_ARG, "grid too large along y for one call");
-            for (int c0 = 0; c0 < nb; c0 += per_launch) {
-                const int cn = std::min(per_launch, nb - c0);
-                FillParams fq = fp;
-                fq.grids = fp.grids + c0;
-                occ_fill8_kernel<<<dim3((unsigned)mz, (unsigned)my, (unsigned)(cn << sh)), FILL_THREADS, 0, st>>>(fq, tile_total);
-                if (c0 + per_launch < nb) MKB_LAUNCHED(h);
-            }
-        } else if (C <= 8) occ_fill_kernel<8><<<grid, FILL_THREADS, 0, st>>>(fp);
+        h->last_kernel = "occ_fill_kernel";
+        if (C <= 8) occ_fill_kernel<8><<<grid, FILL_THREADS, 0, st>>>(fp);
         else if (C <= 16) occ_fill_kernel<16><<<grid, FILL_THREADS, 0, st>>>(fp);
         else occ_fill_kernel<32><<<grid, FILL_THREADS, 0, st>>>(fp);
         MKB_LAUNCHED(h);

@@ -25,21 +25,21 @@ def _run(vd, coords, chans, *, layout, elements=None, radii=None, boxsize=None, 
     return batch, batch.run(d_c, d_ch, layout=layout).cpu().numpy()
 
 
-@pytest.mark.parametrize("case", ["warp_1A", "tile_05A", "generic_12ch", "c5_nonvec", "ragged"])
+@pytest.mark.parametrize("case", ["runs_1A", "runs_05A", "generic_12ch", "v6_c5", "runs_ragged"])
 def test_cxyz_layout_is_a_bit_exact_permutation(case):
     """MKB_OCC_LAYOUT_CXYZ in every fill kernel: out[b] as (C,X,Y,Z) equals the voxel-major result transposed."""
     from moleculekit_b200.tools import voxeldescriptors as vd
 
     rng = np.random.default_rng(5)
     C, vs, B, box = 8, 1.0, 3, [24, 24, 24]
-    if case == "tile_05A":
+    if case == "runs_05A":
         vs, box = 0.5, [14, 14, 14]
     elif case == "generic_12ch":
         C = 12
-    elif case == "c5_nonvec":
+    elif case == "v6_c5":
         C = 5
     coords, chans, elems = _pockets(rng, B, 300, 20.0, C)
-    if case == "ragged":
+    if case == "runs_ragged":
         kw = dict(buffer=3.0)                       # bounding-box grids of different sizes
         coords = [c[: 100 + 90 * i] for i, c in enumerate(coords)]
         chans = [c[: 100 + 90 * i] for i, c in enumerate(chans)]
@@ -86,7 +86,8 @@ def test_cxyz_accumulate_and_batch_api():
     occ.occupancy_grid_batch(d_c, None, batch.descs, out, accumulate=True, layout="cxyz", radii=d_ch[0], chanmask=d_ch[1],
                              n_channels=8)
     got = batch.as_cxyz(out.cpu().numpy())
-    # accumulate runs the v6 warp kernel, the plain call the run kernel: each within 1e-5 of the oracle, not bit-identical
+    # accumulate runs the v6 warp kernel (occ_fill8v_kernel), the plain call the run kernel (occ_fill_runs_kernel): each
+    # within 1e-5 of the oracle, not bit-identical
     want = np.maximum(np.stack(feats), np.float32(0.5))
     assert np.array_equal(got == 0.5, want == 0.5)
     assert np.allclose(got, want, rtol=1.5e-5, atol=0)

@@ -22,10 +22,6 @@ PATHS = {
     "runs": (),
     "runs_notmap": ("MKB_OCC_NO_TMAP",),
     "v6": ("MKB_OCC_V6",),
-    "warp": ("MKB_OCC_WARP",),
-    "warp32": ("MKB_OCC_WARP32",),
-    "tile": ("MKB_OCC_TILE",),
-    "tile_bulk": ("MKB_OCC_TILE", "MKB_OCC_BULK_STORE"),
     "generic": ("MKB_OCC_GENERIC",),
 }
 
@@ -138,13 +134,13 @@ def _n_floats(descs, Cn):
     return int((descs["out_offset"] + descs["dims"].astype(np.int64).prod(axis=1)).max()) * Cn
 
 
-def _pocket_batch(ou, rng, Cn, uniform, n_per=120):
-    """Three grids at 1 A with ragged dims; grid 0 has its atoms in one corner (most of its blocks empty)."""
+def _pocket_batch(ou, rng, Cn, uniform, n_per=120, vs=1.0):
+    """Three grids at 1 A (or vs) with ragged dims; grid 0 has its atoms in one corner (most of its blocks empty)."""
     dims = [(21, 18, 27)] * 3 if uniform else [(21, 18, 27), (13, 30, 9), (17, 17, 17)]
     coords, sigmas, origins = [], [], []
     for b, dm in enumerate(dims):
         org = rng.uniform(-40, 40, 3).round(3)
-        ext = np.asarray(dm, dtype=np.float64) - 1
+        ext = (np.asarray(dm, dtype=np.float64) - 1) * vs
         if b == 0:
             xyz = _atoms(rng, n_per, org + 1.0, 3.0)            # corner: the far blocks see no atom
         else:
@@ -153,7 +149,7 @@ def _pocket_batch(ou, rng, Cn, uniform, n_per=120):
         sigmas.append(_channels(rng, n_per, Cn))
         origins.append(org)
     off = np.cumsum([0] + [len(c) for c in coords])
-    descs, _ = ou.make_grid_descs(np.array(origins), 1.0, np.array(dims), off)
+    descs, _ = ou.make_grid_descs(np.array(origins), vs, np.array(dims), off)
     return np.concatenate(coords), np.concatenate(sigmas), descs
 
 
@@ -181,7 +177,7 @@ def test_guarded_poisoned_output_every_path(ou, oracle, monkeypatch, path, Cn):
 # ---------------------------------------------------------------------------------------------------------------------
 # 2. mixed voxel sizes in one call
 # ---------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("path", ["runs", "v6", "tile", "generic"])
+@pytest.mark.parametrize("path", ["runs", "v6", "generic"])
 def test_mixed_voxel_sizes_one_call(ou, oracle, monkeypatch, path):
     """Grids at 0.3, 0.5, 1.0 and 1.9 A in one batch (the kernel variant and the list table are chosen for the whole batch
     from its finest grid), two of them with identical dims that differ only in voxel size.  With the run kernel every grid
@@ -212,7 +208,7 @@ def test_mixed_voxel_sizes_one_call(ou, oracle, monkeypatch, path):
             assert np.array_equal(g.reshape(-1).view(np.uint32), single.view(np.uint32)), f"grid {b} differs from its single call"
 
 
-@pytest.mark.parametrize("path", ["runs", "runs_notmap", "v6", "warp32", "tile"])
+@pytest.mark.parametrize("path", ["runs", "runs_notmap", "v6"])
 def test_same_dims_different_voxel_sizes(ou, oracle, monkeypatch, path):
     """Grids with identical dims and contiguous offsets from 0 that differ only in voxel size: the batch is not uniform
     (the uniform launches take the first grid's geometry for all), and every grid equals the oracle."""
@@ -270,7 +266,7 @@ def test_shared_overlapping_empty_ranges_dense_compact_to_host(ou, oracle, monke
         if d["atom_begin"] == d["atom_end"]:
             assert not _grid(dense, d, 8, "xyzc").any()
     # the same through the other kernel selectors: ranges are numbered per grid in K2 as well
-    for path in ("v6", "tile", "generic"):
+    for path in ("v6", "generic"):
         _, alt = _run_grid(ou, coords, sigmas, descs, n, envs=PATHS[path], monkeypatch=monkeypatch)
         for b, d in enumerate(descs):
             _assert_occ_close(_grid(alt, d, 8, "xyzc"), _grid(dense, d, 8, "xyzc").astype(np.float64), rtol=2e-5,
@@ -295,7 +291,7 @@ def test_shared_overlapping_empty_ranges_dense_compact_to_host(ou, oracle, monke
 # 4. out_offset layouts
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("layout", ["xyzc", "cxyz"])
-@pytest.mark.parametrize("path", ["runs", "v6", "tile", "generic"])
+@pytest.mark.parametrize("path", ["runs", "v6", "generic"])
 def test_out_offsets_reversed_with_gaps(ou, monkeypatch, path, layout):
     """Grids stored in reverse order, with poisoned gaps between them and a non-zero first offset: the gaps stay
     untouched and every grid's bytes equal the contiguous call (the uniform batch, TMA tensor store by default)."""
@@ -323,21 +319,43 @@ def test_out_offsets_reversed_with_gaps(ou, monkeypatch, path, layout):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# 5. misaligned output
+# 5. fill kernel dispatch
 # ---------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("layout", ["xyzc", "cxyz"])
-def test_misaligned_output_takes_v6_fallback(ou, oracle, monkeypatch, layout):
-    """An output view 4 bytes past a 16-byte boundary cannot take the run kernel (16-byte stores): the v6 kernel with scalar
-    stores serves it, equal to the oracle, guards intact."""
+# id: (channels, voxel size, accumulate, layout, misaligned output, the fill kernel the input alone selects)
+DISPATCH = {
+    "runs_c8_1A": (8, 1.0, False, "xyzc", False, "occ_fill_runs_kernel"),
+    "runs_c8_03A": (8, 0.3, False, "xyzc", False, "occ_fill_runs_kernel"),        # cutoff 17 voxels: still the run kernel
+    "v6_misaligned_xyzc": (8, 1.0, False, "xyzc", True, "occ_fill8v_kernel"),      # 16-byte stores impossible
+    "v6_misaligned_cxyz": (8, 1.0, False, "cxyz", True, "occ_fill8v_kernel"),
+    "v6_accumulate": (8, 1.0, True, "xyzc", False, "occ_fill8v_kernel"),
+    "v6_c5": (5, 1.0, False, "xyzc", False, "occ_fill8v_kernel"),
+    "generic_accumulate_03A": (8, 0.3, True, "xyzc", False, "occ_fill_kernel"),   # cutoff 15..40 voxels off the run kernel
+    "generic_c5_03A": (5, 0.3, False, "xyzc", False, "occ_fill_kernel"),
+    "generic_misaligned_03A": (8, 0.3, False, "xyzc", True, "occ_fill_kernel"),
+    "generic_c8_012A": (8, 0.12, False, "xyzc", False, "occ_fill_kernel"),        # cutoff 42 voxels: beyond the run kernel
+    "generic_c12_1A": (12, 1.0, False, "xyzc", False, "occ_fill_kernel"),
+}
+
+
+@pytest.mark.parametrize("case", list(DISPATCH))
+def test_fill_kernel_dispatch_table(ou, oracle, monkeypatch, case):
+    """Without a selector the fill kernel follows from the input alone: the run kernel for 8 channels, no accumulate, a
+    16-byte aligned output and a cutoff <= 40 voxels; otherwise the v6 warp kernel for <= 8 channels and a cutoff <= 14
+    voxels, and the generic tile kernel for the rest.  Every case equals the oracle with its guards intact (a uniform
+    batch; accumulate on a zero prefill, misaligned outputs 4 bytes past a 16-byte boundary with scalar stores)."""
     from moleculekit_b200 import _lib
 
+    Cn, vs, accumulate, layout, misaligned, kernel = DISPATCH[case]
     rng = np.random.default_rng(5)
-    coords, sigmas, descs = _pocket_batch(ou, rng, 8, uniform=True)
-    buf, out = _run_grid(ou, coords, sigmas, descs, _n_floats(descs, 8), layout, lead=GUARD + 1, monkeypatch=monkeypatch)
-    assert _lib.last_fill_kernel(_dev().index) == "occ_fill8v_kernel"
-    _assert_guards(buf, lead=GUARD + 1)
+    coords, sigmas, descs = _pocket_batch(ou, rng, Cn, uniform=True, vs=vs)
+    n = _n_floats(descs, Cn)
+    lead = GUARD + 1 if misaligned else GUARD
+    buf, out = _run_grid(ou, coords, sigmas, descs, n, layout, lead=lead, init=np.zeros(n, np.float32) if accumulate else None,
+                         accumulate=accumulate, monkeypatch=monkeypatch)
+    assert _lib.last_fill_kernel(_dev().index) == kernel
+    _assert_guards(buf, lead=lead)
     for b, d in enumerate(descs):
-        _assert_occ_close(_grid(out, d, 8, layout), _want(oracle, d, coords, sigmas), what=f"grid {b}")
+        _assert_occ_close(_grid(out, d, Cn, layout), _want(oracle, d, coords, sigmas), what=f"{case} grid {b}")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -371,12 +389,11 @@ def _check_accumulated(got, prefill, want, reached_val, what):
 
 
 @pytest.mark.parametrize("layout", ["xyzc", "cxyz"])
-@pytest.mark.parametrize("path", ["default", "warp32", "tile", "generic"])
+@pytest.mark.parametrize("path", ["default", "generic"])
 def test_accumulate_prefills_grid_paths(ou, oracle, monkeypatch, path, layout):
     """MKB_OCC_ACCUMULATE follows the reference's update rule on every grid kernel (accumulate calls never take the run
-    kernel: "default" is the v6 kernel, "warp32" the one-voxel-per-lane warp kernel): an entry is updated only when an atom
-    with a non-zero sigma lies within 5 A and its value is larger; NaN sticks; negative prefills stay where no atom
-    reaches."""
+    kernel: "default" is the v6 kernel): an entry is updated only when an atom with a non-zero sigma lies within 5 A and
+    its value is larger; NaN sticks; negative prefills stay where no atom reaches."""
     rng = np.random.default_rng(6)
     coords, sigmas, descs = _pocket_batch(ou, rng, 8, uniform=False)
     envs = () if path == "default" else PATHS[path]
@@ -422,7 +439,7 @@ def test_accumulate_prefills_points(ou, oracle, Cn):
 CHUNK_CASES = {
     "c4_v6": (4, 8, ()),                 # warp kernel: 16 383 grids per launch (8-voxel x extent); block totals at 65 535
     "c8_runs": (8, 8, ()),               # persistent run kernel over the whole batch
-    "c8_tile": (8, 8, ("MKB_OCC_TILE",)),  # tile kernels: 65 535 grids per launch
+    "c8_generic": (8, 8, ("MKB_OCC_GENERIC",)),  # tile kernel, 8 channels: 65 535 grids per launch
     "c12_generic": (12, 4, ()),          # generic kernel: 65 535 grids per launch
 }
 
@@ -528,7 +545,7 @@ def test_scratch_reuse_large_tiny_medium_large(ou, oracle, monkeypatch):
 # 9. degenerate shapes and bad descriptors
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("layout", ["xyzc", "cxyz"])
-@pytest.mark.parametrize("path", ["runs", "v6", "warp32", "tile", "generic"])
+@pytest.mark.parametrize("path", ["runs", "v6", "generic"])
 def test_degenerate_shapes(ou, oracle, monkeypatch, path, layout):
     """1x1x1, 1x1xN and Nx1x1 grids, a grid whose atoms all sit beyond the 5 A halo and a grid without atoms, in one call."""
     rng = np.random.default_rng(9)
@@ -663,7 +680,7 @@ def test_small_radii_bitmask_channels(ou, oracle, layout, accumulate):
         _assert_occ_close(g, want, what=f"{layout} grid {b}")
 
 
-@pytest.mark.parametrize("path", ["runs", "v6", "tile", "generic", "points"])
+@pytest.mark.parametrize("path", ["runs", "v6", "generic", "points"])
 @pytest.mark.parametrize("sigma", SIGMAS)
 def test_sigma_sweep(ou, oracle, monkeypatch, path, sigma):
     """Channel sigmas from 0.05 to 100 A and a negative one (the reference squares x, so -1.7 acts as 1.7): equal to the

@@ -121,7 +121,7 @@ def test_channel_counts_and_multisigma(vd, oracle, C):
     _assert_occ_close(feats, want)
 
 
-@pytest.mark.parametrize("vs", [0.3, 0.4, 0.5, 0.7, 1.0, 1.9, 2.6])  # 0.3: tile kernel (halo rows exceed a warp), 0.4-1.0: 2x4x8 block kernel
+@pytest.mark.parametrize("vs", [0.3, 0.4, 0.5, 0.7, 1.0, 1.9, 2.6])  # the run kernel at every size (cutoff <= 40 voxels)
 def test_voxel_sizes_buffer_mode(vd, oracle, vs):
     from moleculekit_b200.molecule_lite import MolLite
 
@@ -192,15 +192,13 @@ def test_full_size_c3_properties(vd, oracle):
         _assert_occ_close(out[offs[b]:offs[b + 1]].cpu().numpy(), want)
 
 
-@pytest.mark.parametrize("envs", [("MKB_OCC_TILE",), ("MKB_OCC_TILE", "MKB_OCC_BULK_STORE"), ("MKB_OCC_GENERIC",), ("MKB_OCC_WARP",),
-                                  ("MKB_OCC_WARP32",), ("MKB_OCC_NO_TMAP",)])
+@pytest.mark.parametrize("envs", [("MKB_OCC_GENERIC",), ("MKB_OCC_V6",), ("MKB_OCC_NO_TMAP",)])
 def test_alternative_kernel_paths_agree(vd, monkeypatch, envs):
     """MKB_OCC_NO_TMAP: the default run kernel with 16 bulk row copies per block instead of one TMA tensor store (the route of
     non-uniform batches and of the compact / to-host transfers; the grid dims here are not multiples of the 4 x 4 x 8 block, so
     the tensor store is clipped by the TMA unit and the row copies by hand).
-    The tile kernel (quarter lists), its opt-in TMA bulk-store epilogue, the generic tile kernel and the one-voxel-per-lane
-    warp kernel (2x4x4 blocks) agree with the default two-voxels-per-lane warp kernel (ragged grid: dims not multiples of
-    the block / tile sizes)."""
+    The generic tile kernel and the v6 warp kernel (2x4x8 blocks, two voxels per lane) agree with the default run kernel
+    (ragged grid: dims not multiples of the block / tile sizes)."""
     from moleculekit_b200 import workloads
 
     w = workloads.protein_pockets(B=2, n_atoms=700, box=37.0, radius=12.0, seed=21)
