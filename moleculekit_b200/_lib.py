@@ -1,11 +1,13 @@
-"""ctypes binding of libmkb200.so (include/mkb200.h).  No CPU fallback: if the CUDA library is missing or
-no CUDA device is present, every entry point raises."""
+"""ctypes binding of libmkb200.so (include/mkb200.h) and the one path by which the modules call it with torch tensors
+(:func:`call`, :func:`traj`, :func:`ptr`).  No CPU fallback: if the CUDA library is missing or no CUDA device is
+present, every entry point raises."""
 from __future__ import annotations
 
 import ctypes as C
 import os
 
 import numpy as np
+import torch
 
 PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(PKG, "lib", "libmkb200.so")
@@ -159,6 +161,100 @@ def check(rc: int, h) -> None:
     if rc != MKB_OK:
         msg = load().mkb_last_error(h)
         raise (MkbUnsupported if rc == -5 else MkbError)(f"libmkb200 status {rc}: {msg.decode() if msg else '?'}")
+
+
+# ------------------------------------------------------------------------------------------ calls from torch tensors
+def device(device):
+    """The torch.device a host-level function runs on: ``device``, or torch's current CUDA device for None."""
+    if device is None:
+        if not torch.cuda.is_available():
+            raise MkbError("moleculekit_b200 needs a CUDA device (there is no CPU fallback)")
+        return torch.device("cuda", torch.cuda.current_device())
+    d = torch.device(device)
+    if d.type != "cuda":
+        raise MkbError(f"moleculekit_b200 runs on CUDA devices only, got {d}")
+    return torch.device("cuda", d.index if d.index is not None else torch.cuda.current_device())
+
+
+def tensor_device(t, caller: str):
+    """The device of ``t``, which must be a CUDA device: ``caller`` names the entry point in the error."""
+    dev = t.device
+    if dev.type != "cuda":
+        raise MkbError(f"{caller} runs on CUDA tensors only, got {dev} (there is no CPU fallback)")
+    return dev
+
+
+def ptr(t) -> C.c_void_p:
+    """The data pointer of a tensor; None gives NULL."""
+    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+
+
+def stream(dev) -> C.c_void_p:
+    """torch's current stream on ``dev``: every entry point is ordered on it."""
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def index_arg(t, dev, dtype=torch.int32, cols: int | None = None) -> None:
+    """Assert that the index tensor ``t`` (None passes) is a contiguous ``dtype`` tensor on ``dev``, 1-D or, with
+    ``cols``, (m, cols).  The library reads packed 32-bit indices: an int64 tensor would be read as pairs of words."""
+    if t is None:
+        return
+    assert t.dtype == dtype and t.device == dev and t.is_contiguous(), \
+        f"index tensors must be contiguous {dtype} on {dev}, got {t.dtype} on {t.device}"
+    assert t.ndim == 1 if cols is None else (t.ndim == 2 and t.shape[1] == cols), f"bad index tensor shape {tuple(t.shape)}"
+
+
+def traj(coords, box=None, writable: bool = False) -> Traj:
+    """`mkb_traj` view of an (N, 3, F) float32 CUDA trajectory and its (3, F) float32 ``box`` (None: a NULL box).
+
+    A frame-minor tensor -- contiguous, or a frame slice of a contiguous one -- is passed in place.  Any other layout is
+    copied for reading, kept alive on the struct; with ``writable`` (an entry point that writes ``coords``) it raises
+    ValueError instead, as the result would land in the copy."""
+    assert coords.is_cuda and coords.dtype == torch.float32 and coords.ndim == 3 and coords.shape[1] == 3
+    N, _, F = coords.shape
+    s_atom, s_axis, s_frame = coords.stride()
+    if not (N == 0 or (s_atom == 3 * s_axis and (F <= 1 or s_frame == 1) and s_axis >= F)):
+        if writable:
+            raise ValueError("coords must be (N, 3, F) frame-minor (a frame slice of a contiguous trajectory is fine)")
+        coords = coords.contiguous()
+        s_axis = coords.stride(1)
+    t = Traj()
+    t.n_atoms, t.n_frames = N, F
+    t.frame_stride = t.frame_stride_box = max(s_axis if N else F, F, 1)
+    if box is not None:
+        assert box.is_cuda and box.dtype == torch.float32 and box.ndim == 2 and box.shape[0] == 3
+        if F <= 1:
+            # the stride of a size-1 / empty dimension is meaningless (numpy views may carry 0): normalise
+            box = box.contiguous()
+            t.frame_stride_box = max(F, 1)
+        else:
+            s_box, s_unit = box.stride()
+            assert s_unit == 1, "box must be (3, F) frame-minor (a frame slice of a contiguous one is fine)"
+            t.frame_stride_box = s_box
+        t.box = box.data_ptr()
+    t.coords = coords.data_ptr()
+    t._keepalive = (coords, box)  # a copy made here must outlive the launch
+    return t
+
+
+def call(dev, name: str, *args) -> None:
+    """Run the entry point ``name`` as name(handle, stream, *args) on CUDA device ``dev`` and torch's current stream
+    there; a failed status raises :class:`MkbError`."""
+    h = handle(dev.index)
+    with torch.cuda.device(dev):
+        check(getattr(load(), name)(h, stream(dev), *args), h)
+
+
+def count_fill(dev, count_name: str, fill_name: str, args: tuple, offsets, alloc) -> tuple:
+    """The two-pass entry points: ``count_name(*args, offsets, &total)`` writes the row offsets and returns the total
+    (read back: synchronises), ``alloc(total)`` returns the output tensors and, when total > 0,
+    ``fill_name(*args, offsets, *outputs)`` fills them.  Returns the outputs."""
+    total = C.c_int64(0)
+    call(dev, count_name, *args, ptr(offsets), C.byref(total))
+    outs = alloc(max(total.value, 0))
+    if total.value > 0:
+        call(dev, fill_name, *args, ptr(offsets), *map(ptr, outs))
+    return outs
 
 
 def launch_count(device: int = 0) -> int:

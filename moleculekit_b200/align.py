@@ -23,30 +23,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .distance_utils import _ptr
-from .occupancy_utils import _dev, _stream_ptr
 
 RECORD = 16  # doubles per frame record: R (row-major, x' = R (x - p) + q), p_bar, q_bar, pad
-
-
-def _traj(coords: torch.Tensor, writable: bool = False) -> _lib.Traj:
-    """`mkb_traj` view (no box) of an (N, 3, F) float32 frame-minor tensor or a frame slice of one."""
-    assert coords.is_cuda and coords.dtype == torch.float32 and coords.ndim == 3 and coords.shape[1] == 3
-    N, _, F = coords.shape
-    framed = N == 0 or (coords.stride(0) == 3 * coords.stride(1) and (F <= 1 or coords.stride(2) == 1)
-                        and coords.stride(1) >= F)
-    if not framed:
-        if writable:
-            raise ValueError("coords must be (N, 3, F) frame-minor (a frame slice of a contiguous trajectory is fine)")
-        coords = coords.contiguous()
-    t = _lib.Traj()
-    t.n_atoms, t.n_frames = N, F
-    t.frame_stride = max(coords.stride(1) if N else F, F, 1)
-    t.frame_stride_box = t.frame_stride
-    t.coords = coords.data_ptr()
-    t.box = None
-    t._keepalive = coords
-    return t
 
 
 # ---------------------------------------------------------------------------------------------- device level
@@ -55,52 +33,47 @@ def superpose_device(coords, sel, refcoords, refsel, frames=None):
     (M, 3, 1): one reference frame, or (M, 3, F): frame f onto reference frame f.  ``sel`` / ``refsel`` / ``frames``
     are int32 CUDA tensors (``frames`` None = all frames).  Returns (records (n, 16) float64, status (n,) int32); row k
     belongs to frame ``frames[k]``; status 1 = non-finite coordinates in the selection."""
-    dev = coords.device
+    dev = _lib.tensor_device(coords, "superpose_device")
+    for x in (sel, refsel, frames):
+        _lib.index_arg(x, dev)
     if int(sel.numel()) != int(refsel.numel()):
         raise ValueError(f"selections differ in size: {int(sel.numel())} and {int(refsel.numel())}")
     n = coords.shape[2] if frames is None else int(frames.numel())
     records = torch.empty((n, RECORD), dtype=torch.float64, device=dev)
     status = torch.empty(n, dtype=torch.int32, device=dev)
-    h = _lib.handle(dev.index)
-    t, r = _traj(coords), _traj(refcoords)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_align_fit(h, _stream_ptr(dev), C.byref(t), _ptr(sel), C.byref(r), _ptr(refsel),
-                                       int(sel.numel()), _ptr(frames), n, _ptr(records), _ptr(status))
-    _lib.check(rc, h)
+    t, r = _lib.traj(coords), _lib.traj(refcoords)
+    _lib.call(dev, "mkb_align_fit", C.byref(t), _lib.ptr(sel), C.byref(r), _lib.ptr(refsel), int(sel.numel()),
+              _lib.ptr(frames), n, _lib.ptr(records), _lib.ptr(status))
     return records, status
 
 
 def apply_device(coords, records, frames=None, status=None):
     """Superpose the listed frames of ``coords`` IN PLACE with the records of :func:`superpose_device` (frames whose
     ``status`` is not 0 are left as they are) and return ``coords``."""
-    dev = coords.device
+    dev = _lib.tensor_device(coords, "apply_device")
+    _lib.index_arg(frames, dev)
     n = coords.shape[2] if frames is None else int(frames.numel())
     assert records.dtype == torch.float64 and tuple(records.shape) == (n, RECORD) and records.is_contiguous()
-    h = _lib.handle(dev.index)
-    t = _traj(coords, writable=True)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_align_apply(h, _stream_ptr(dev), C.byref(t), _ptr(frames), n, _ptr(records),
-                                         _ptr(status))
-    _lib.check(rc, h)
+    t = _lib.traj(coords, writable=True)
+    _lib.call(dev, "mkb_align_apply", C.byref(t), _lib.ptr(frames), n, _lib.ptr(records), _lib.ptr(status))
     return coords
 
 
 def rmsd_device(coords, sel, refcoords, refsel, records=None, frames=None):
     """Per listed frame, sqrt(mean |T(x) - q|^2) over the selections as float32 (n,); T = the frame's fit record, or
     no transform when ``records`` is None.  The trajectory is not modified."""
-    dev = coords.device
+    dev = _lib.tensor_device(coords, "rmsd_device")
+    for x in (sel, refsel, frames):
+        _lib.index_arg(x, dev)
     if int(sel.numel()) != int(refsel.numel()):
         raise ValueError(f"selections differ in size: {int(sel.numel())} and {int(refsel.numel())}")
     n = coords.shape[2] if frames is None else int(frames.numel())
     if records is not None:
         assert records.dtype == torch.float64 and tuple(records.shape) == (n, RECORD) and records.is_contiguous()
     out = torch.empty(n, dtype=torch.float32, device=dev)
-    h = _lib.handle(dev.index)
-    t, r = _traj(coords), _traj(refcoords)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_rmsd(h, _stream_ptr(dev), C.byref(t), _ptr(sel), C.byref(r), _ptr(refsel),
-                                  int(sel.numel()), _ptr(frames), n, _ptr(records), _ptr(out))
-    _lib.check(rc, h)
+    t, r = _lib.traj(coords), _lib.traj(refcoords)
+    _lib.call(dev, "mkb_rmsd", C.byref(t), _lib.ptr(sel), C.byref(r), _lib.ptr(refsel), int(sel.numel()),
+              _lib.ptr(frames), n, _lib.ptr(records), _lib.ptr(out))
     return out
 
 
@@ -160,7 +133,7 @@ def align(mol, sel, refmol=None, refsel=None, frames=None, matchingframes=False,
     fl = None if frames is None else _frame_list(frames, F)
     if F == 0 or (fl is not None and fl.size == 0):
         return
-    dev = _dev(device)
+    dev = _lib.device(device)
     d = torch.from_numpy(np.ascontiguousarray(mol.coords, dtype=np.float32)).to(dev)
     if refmol is mol:
         ref = d if matchingframes else d[:, :, int(mol.frame):int(mol.frame) + 1]
@@ -191,7 +164,7 @@ def molRMSD(mol, refmol, rmsdsel1, rmsdsel2, device=None):
         raise ValueError(f"the reference has {Fr} frames: 1 or the molecule's {F}")
     if F == 0:
         return np.zeros(0, np.float32)
-    dev = _dev(device)
+    dev = _lib.device(device)
     x = torch.from_numpy(np.ascontiguousarray(mol.coords[i1], dtype=np.float32)).to(dev)
     q = torch.from_numpy(np.ascontiguousarray(refmol.coords[i2], dtype=np.float32)).to(dev)
     ar = torch.arange(i1.size, dtype=torch.int32, device=dev)

@@ -11,14 +11,11 @@ The reference loops over all (query, source) pairs; `mkb_within_distance` bins t
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 import torch
 
 from . import _lib
-from .distance_utils import _check, _ptr
-from .occupancy_utils import _dev, _stream_ptr
+from .distance_utils import _check
 
 
 def within_distance_device(coords: torch.Tensor, cutoff: float, sel2: torch.Tensor, sel1: torch.Tensor | None = None,
@@ -32,11 +29,8 @@ def within_distance_device(coords: torch.Tensor, cutoff: float, sel2: torch.Tens
     if results is None:
         results = torch.zeros(n1, dtype=torch.bool, device=dev)
     assert results.dtype == torch.bool and results.is_contiguous() and results.numel() == n1
-    h = _lib.handle(dev.index)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_within_distance(h, _stream_ptr(dev), _ptr(coords), int(coords.shape[0]), _ptr(sel1), n1,
-                                             _ptr(sel2), int(sel2.numel()), float(np.float32(cutoff)), _ptr(results))
-    _lib.check(rc, h)
+    _lib.call(dev, "mkb_within_distance", _lib.ptr(coords), int(coords.shape[0]), _lib.ptr(sel1), n1, _lib.ptr(sel2),
+              int(sel2.numel()), float(np.float32(cutoff)), _lib.ptr(results))
     return results
 
 
@@ -54,7 +48,7 @@ def within_distance(coords, cutoff, sel1, sel2, sel2_min_coords, sel2_max_coords
     n = coords.shape[0]
     if int(sel1.max()) >= n or int(sel2.max()) >= n:
         raise IndexError("atom index out of range")
-    dev = _dev(device)
+    dev = _lib.device(device)
     d_coords = torch.from_numpy(np.ascontiguousarray(coords[:, :3])).to(dev)
     d1 = torch.from_numpy(np.ascontiguousarray(sel1).view(np.int32)).to(dev)
     d2 = torch.from_numpy(np.ascontiguousarray(sel2).view(np.int32)).to(dev)

@@ -8,14 +8,12 @@ reference's own test compares in -- rather than in the reference's box-traversal
 """
 from __future__ import annotations
 
-import ctypes as C
 import logging
 
 import numpy as np
 import torch
 
 from . import _lib
-from .occupancy_utils import _dev, _stream_ptr
 
 logger = logging.getLogger(__name__)
 
@@ -107,22 +105,15 @@ def bond_grid_search(coords: np.ndarray, grid_cutoff: float, is_hydrogen: np.nda
             "all the bonds in Molecule pass `guessBonds=False` to the function or perform "
             "the bond guessing on a wrapped frame."
         )
-    dev = _dev(device)
+    dev = _lib.device(device)
     d_c = torch.from_numpy(coords).to(dev)
     d_r = torch.from_numpy(np.ascontiguousarray(radii, dtype=np.float32)).to(dev)
     d_h = torch.from_numpy(np.ascontiguousarray(is_hydrogen, dtype=np.uint32).view(np.int32)).to(dev)
     off = torch.empty(n + 1, dtype=torch.int64, device=dev)
-    total = C.c_int64(0)
-    h = _lib.handle(dev.index)
-    p = lambda t: C.c_void_p(t.data_ptr())
-    pd32 = float(np.float32(pairdist))
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_bonds_count(h, _stream_ptr(dev), p(d_c), p(d_r), p(d_h), n, pd32, p(off), C.byref(total))
-        _lib.check(rc, h)
-        if total.value == 0:
-            return np.zeros((0, 2), dtype=np.uint32)
-        pairs = torch.empty((total.value, 2), dtype=torch.int32, device=dev)
-        rc = _lib.load().mkb_bonds_fill(h, _stream_ptr(dev), p(d_c), p(d_r), p(d_h), n, pd32, p(off), p(pairs))
-        _lib.check(rc, h)
+    args = (_lib.ptr(d_c), _lib.ptr(d_r), _lib.ptr(d_h), n, float(np.float32(pairdist)))
+    (pairs,) = _lib.count_fill(dev, "mkb_bonds_count", "mkb_bonds_fill", args, off,
+                               lambda total: (torch.empty((total, 2), dtype=torch.int32, device=dev),))
+    if pairs.shape[0] == 0:
+        return np.zeros((0, 2), dtype=np.uint32)
     out = pairs.cpu().numpy().view(np.uint32)
     return out[np.lexsort((out[:, 1], out[:, 0]))]  # rows are (i < j); canonical order

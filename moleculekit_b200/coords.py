@@ -18,9 +18,7 @@ import ctypes as C
 import torch
 
 from . import _lib
-from .align import RECORD, _traj
-from .distance_utils import _ptr
-from .occupancy_utils import _stream_ptr
+from .align import RECORD
 
 
 def _check_records(records, n):
@@ -42,7 +40,9 @@ def coordinates_device(coords, sel, records=None, frames=None, out=None):
     """(n, 3k) float32: row r = the aligned coordinates of the ``sel`` atoms in listed frame r, all X of the selection in
     selection order, then all Y, then all Z.  ``out`` (optional) receives them, e.g. a frame shard's rows of a whole
     trajectory's matrix."""
-    dev = coords.device
+    dev = _lib.tensor_device(coords, "coordinates_device")
+    _lib.index_arg(sel, dev)
+    _lib.index_arg(frames, dev)
     k = int(sel.numel())
     n = coords.shape[2] if frames is None else int(frames.numel())
     _check_records(records, n)
@@ -50,12 +50,9 @@ def coordinates_device(coords, sel, records=None, frames=None, out=None):
     if n == 0:  # an empty frame list has a NULL data pointer, which the library reads as "every frame"
         return out
     ld = max(out.stride(0) if n > 1 else 3 * k, 3 * k)
-    h = _lib.handle(dev.index)
-    t = _traj(coords)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_coordinates(h, _stream_ptr(dev), C.byref(t), _ptr(sel), k, _ptr(frames), n,
-                                         _ptr(records), _ptr(out), ld)
-    _lib.check(rc, h)
+    t = _lib.traj(coords)
+    _lib.call(dev, "mkb_coordinates", C.byref(t), _lib.ptr(sel), k, _lib.ptr(frames), n, _lib.ptr(records),
+              _lib.ptr(out), ld)
     return out
 
 
@@ -63,19 +60,18 @@ def coord_sums_device(coords, sel, records=None, frames=None):
     """(k, 3) float64: per selected atom and axis, the sum over the listed frames of the aligned float32 coordinate.  The
     summation order depends only on the selection and the ordered frame list (fixed chunks of 64 frames, added in
     order), so repeated calls, a frame slice and the equivalent explicit list give the same bits."""
-    dev = coords.device
+    dev = _lib.tensor_device(coords, "coord_sums_device")
+    _lib.index_arg(sel, dev)
+    _lib.index_arg(frames, dev)
     k = int(sel.numel())
     n = coords.shape[2] if frames is None else int(frames.numel())
     _check_records(records, n)
     sums = torch.empty((k, 3), dtype=torch.float64, device=dev)
     if n == 0:
         return sums.zero_()
-    h = _lib.handle(dev.index)
-    t = _traj(coords)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_coord_sums(h, _stream_ptr(dev), C.byref(t), _ptr(sel), k, _ptr(frames), n,
-                                        _ptr(records), _ptr(sums))
-    _lib.check(rc, h)
+    t = _lib.traj(coords)
+    _lib.call(dev, "mkb_coord_sums", C.byref(t), _lib.ptr(sel), k, _lib.ptr(frames), n, _lib.ptr(records),
+              _lib.ptr(sums))
     return sums
 
 
@@ -84,23 +80,20 @@ def fluctuation_device(coords, sel, centre, records=None, frames=None, groups=No
     coordinate and ``centre`` a (k, 3) float64 CUDA tensor (the mean or a reference structure): (n, k) float32.  With
     ``groups`` (G + 1,) int64 offsets over selection positions (0 first, k last, nondecreasing, no empty group) the
     result is (n, G): the float64 mean of each group's per-atom values, rounded once."""
-    dev = coords.device
+    dev = _lib.tensor_device(coords, "fluctuation_device")
+    _lib.index_arg(sel, dev)
+    _lib.index_arg(frames, dev)
+    _lib.index_arg(groups, dev, torch.int64)
     k = int(sel.numel())
     n = coords.shape[2] if frames is None else int(frames.numel())
     _check_records(records, n)
     assert centre.dtype == torch.float64 and tuple(centre.shape) == (k, 3) and centre.is_contiguous()
-    G = k
-    if groups is not None:
-        assert groups.dtype == torch.int64 and groups.ndim == 1 and groups.is_contiguous()
-        G = int(groups.numel()) - 1
+    G = k if groups is None else int(groups.numel()) - 1
     out = _rows(out, n, G, torch.float32, dev)
     if n == 0:
         return out
     ld = max(out.stride(0) if n > 1 else G, G)
-    h = _lib.handle(dev.index)
-    t = _traj(coords)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_fluctuation(h, _stream_ptr(dev), C.byref(t), _ptr(sel), k, _ptr(frames), n,
-                                         _ptr(records), _ptr(centre), _ptr(groups), G, _ptr(out), ld)
-    _lib.check(rc, h)
+    t = _lib.traj(coords)
+    _lib.call(dev, "mkb_fluctuation", C.byref(t), _lib.ptr(sel), k, _lib.ptr(frames), n, _lib.ptr(records),
+              _lib.ptr(centre), _lib.ptr(groups), G, _lib.ptr(out), ld)
     return out

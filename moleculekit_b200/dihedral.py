@@ -16,10 +16,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .align import _traj
 from .coords import _rows
-from .distance_utils import _ptr
-from .occupancy_utils import _stream_ptr
 
 
 def dihedralAngle(pos) -> float:
@@ -52,24 +49,17 @@ def dihedrals_device(coords, quads, sincos, frames=None, out=None):
     atoms) gives angle 0 and (sin, cos) = (0, 1); a non-finite coordinate gives NaN.  ``frames`` must be an int32
     tensor on the trajectory's device.  ``out`` (optional) receives the rows, e.g. a frame shard's rows of a whole
     trajectory's matrix (unit column stride, any row stride)."""
-    dev = coords.device
-    if dev.type != "cuda":
-        raise _lib.MkbError(f"dihedrals_device runs on CUDA tensors only, got {dev} (there is no CPU fallback)")
-    assert quads.dtype == torch.int32 and quads.ndim == 2 and quads.shape[1] == 4 and quads.is_contiguous()
-    assert quads.device == dev
+    dev = _lib.tensor_device(coords, "dihedrals_device")
+    _lib.index_arg(quads, dev, cols=4)
+    _lib.index_arg(frames, dev)
     m = int(quads.shape[0])
     nv = 2 if sincos else 1
-    if frames is not None:
-        assert frames.dtype == torch.int32 and frames.device == dev and frames.ndim == 1 and frames.is_contiguous()
     n = coords.shape[2] if frames is None else int(frames.numel())
     out = _rows(out, n, nv * m, torch.float32, dev)
     if n == 0:  # an empty frame list has a NULL data pointer, which the library reads as "every frame"
         return out
     ld = max(out.stride(0) if n > 1 else nv * m, nv * m)
-    h = _lib.handle(dev.index)
-    t = _traj(coords)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_dihedrals(h, _stream_ptr(dev), C.byref(t), _ptr(quads), m, _ptr(frames), n,
-                                       1 if sincos else 0, _ptr(out), ld)
-    _lib.check(rc, h)
+    t = _lib.traj(coords)
+    _lib.call(dev, "mkb_dihedrals", C.byref(t), _lib.ptr(quads), m, _lib.ptr(frames), n, 1 if sincos else 0,
+              _lib.ptr(out), ld)
     return out

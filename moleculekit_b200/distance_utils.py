@@ -14,37 +14,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .occupancy_utils import _dev, _stream_ptr
 
 _NAN = float("nan")
-
-
-def _traj(coords: torch.Tensor, box: torch.Tensor) -> _lib.Traj:
-    """`mkb_traj` view of a (N, 3, F) frame-minor trajectory (contiguous, or a frame slice of a contiguous one)."""
-    assert coords.is_cuda and box.is_cuda and coords.dtype == torch.float32 and box.dtype == torch.float32
-    assert coords.ndim == 3 and coords.shape[1] == 3 and box.ndim == 2 and box.shape[0] == 3
-    N, _, F = coords.shape
-    t = _lib.Traj()
-    t.n_atoms, t.n_frames = N, F
-    if F <= 1 or N == 0:
-        # strides of size-1 / empty dimensions are meaningless (numpy views may carry 0): normalise
-        coords = coords.contiguous()
-        box = box.contiguous()
-        t.frame_stride = max(F, 1)
-        t.frame_stride_box = max(F, 1)
-    else:
-        assert coords.stride(2) == 1 and coords.stride(0) == 3 * coords.stride(1) and box.stride(1) == 1, \
-            "coords must be (N, 3, F) frame-minor (a frame slice of a contiguous trajectory is fine)"
-        t.frame_stride = coords.stride(1)
-        t.frame_stride_box = box.stride(0)
-    t.coords = coords.data_ptr()
-    t.box = box.data_ptr()
-    t._keepalive = (coords, box)  # the normalised copies must outlive the launch
-    return t
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
 def n_columns(n1: int, n2: int, selfdist: bool) -> int:
@@ -64,14 +35,10 @@ def dist_trajectory_device(coords, box, sel1, sel2, chains, selfdist: bool, pbc:
     mode = _lib.DIST_CONTACTS if metric == "contacts" else (_lib.DIST_DISTANCES if exact else _lib.DIST_DISTANCES_FAST)
     if out is None:
         out = torch.empty((F, P), dtype=torch.uint8 if mode == _lib.DIST_CONTACTS else torch.float32, device=dev)  # the kernel writes every element
-    h = _lib.handle(dev.index)
-    tr = _traj(coords, box)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_dist_trajectory(
-            h, _stream_ptr(dev), C.byref(tr), _ptr(sel1), len(sel1), _ptr(sel2), len(sel2), _ptr(chains),
-            int(bool(selfdist)), int(bool(pbc)), mode, _NAN if truncate is None else float(truncate),
-            float(threshold), _ptr(out))
-    _lib.check(rc, h)
+    tr = _lib.traj(coords, box)
+    _lib.call(dev, "mkb_dist_trajectory", C.byref(tr), _lib.ptr(sel1), len(sel1), _lib.ptr(sel2), len(sel2),
+              _lib.ptr(chains), int(bool(selfdist)), int(bool(pbc)), mode, _NAN if truncate is None else float(truncate),
+              float(threshold), _lib.ptr(out))
     return out.view(torch.bool) if mode == _lib.DIST_CONTACTS else out
 
 
@@ -79,19 +46,12 @@ def contacts_trajectory_device(coords, box, sel1, sel2, chains, selfdist: bool, 
     """K4 on CUDA tensors.  Returns (frame_offsets (F+1,) int64 cuda, pairs (total, 2) uint32-as-int32 cuda)."""
     dev = coords.device
     F, n1 = coords.shape[2], len(sel1)
-    h = _lib.handle(dev.index)
-    tr = _traj(coords, box)
+    tr = _lib.traj(coords, box)
     row_off = torch.empty(F * n1 + 1, dtype=torch.int64, device=dev)
-    total = C.c_int64(0)
-    args = (C.byref(tr), _ptr(sel1), n1, _ptr(sel2), len(sel2), _ptr(chains), int(bool(selfdist)), int(bool(pbc)),
-            float(np.float32(dist_threshold)))
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_contacts_count(h, _stream_ptr(dev), *args, _ptr(row_off), C.byref(total))
-        _lib.check(rc, h)
-        pairs = torch.empty((max(total.value, 0), 2), dtype=torch.int32, device=dev)
-        if total.value > 0:
-            rc = _lib.load().mkb_contacts_fill(h, _stream_ptr(dev), *args, _ptr(row_off), _ptr(pairs))
-            _lib.check(rc, h)
+    args = (C.byref(tr), _lib.ptr(sel1), n1, _lib.ptr(sel2), len(sel2), _lib.ptr(chains), int(bool(selfdist)),
+            int(bool(pbc)), float(np.float32(dist_threshold)))
+    (pairs,) = _lib.count_fill(dev, "mkb_contacts_count", "mkb_contacts_fill", args, row_off,
+                               lambda total: (torch.empty((total, 2), dtype=torch.int32, device=dev),))
     frame_off = row_off[::n1] if n1 > 0 else torch.zeros(F + 1, dtype=torch.int64, device=dev)
     return frame_off.contiguous(), pairs
 
@@ -102,14 +62,10 @@ def shell_counts_device(coords, box, sel1, sel2, chains, selfdist: bool, pbc: bo
     F, n1 = coords.shape[2], len(sel1)
     numshells = int(edges.shape[0]) - 1
     counts = torch.zeros((F, n1, numshells), dtype=torch.int32, device=dev)
-    h = _lib.handle(dev.index)
-    tr = _traj(coords, box)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_shell_counts(
-            h, _stream_ptr(dev), C.byref(tr), _ptr(sel1), n1, _ptr(sel2), len(sel2), _ptr(chains),
-            int(bool(selfdist)), int(bool(pbc)), _NAN if truncate is None else float(truncate), _ptr(edges), numshells,
-            _ptr(counts))
-    _lib.check(rc, h)
+    tr = _lib.traj(coords, box)
+    _lib.call(dev, "mkb_shell_counts", C.byref(tr), _lib.ptr(sel1), n1, _lib.ptr(sel2), len(sel2), _lib.ptr(chains),
+              int(bool(selfdist)), int(bool(pbc)), _NAN if truncate is None else float(truncate), _lib.ptr(edges),
+              numshells, _lib.ptr(counts))
     return counts
 
 
@@ -149,14 +105,11 @@ def dist_reduction_device(coords, box, groups1, groups2, gchains1, gchains2, sel
     out = torch.zeros((F, P), dtype=torch.uint8 if mode else torch.float32, device=dev)
     o1, a1 = _groups_csr(groups1, dev)
     o2, a2 = _groups_csr(groups2, dev)
-    h = _lib.handle(dev.index)
-    tr = _traj(coords, box)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_dist_reduction(
-            h, _stream_ptr(dev), C.byref(tr), _ptr(o1), _ptr(a1), G1, _ptr(o2), _ptr(a2), G2, _ptr(gchains1),
-            _ptr(gchains2), int(bool(selfdist)), int(bool(pbc)), _ptr(masses), int(red1), int(red2), int(bool(pairs)),
-            mode, _NAN if truncate is None else float(truncate), float(threshold), _ptr(out))
-    _lib.check(rc, h)
+    tr = _lib.traj(coords, box)
+    _lib.call(dev, "mkb_dist_reduction", C.byref(tr), _lib.ptr(o1), _lib.ptr(a1), G1, _lib.ptr(o2), _lib.ptr(a2), G2,
+              _lib.ptr(gchains1), _lib.ptr(gchains2), int(bool(selfdist)), int(bool(pbc)), _lib.ptr(masses), int(red1),
+              int(red2), int(bool(pairs)), mode, _NAN if truncate is None else float(truncate), float(threshold),
+              _lib.ptr(out))
     return out.view(torch.bool) if mode else out
 
 
@@ -171,7 +124,7 @@ def _check(name, arr, dtype, ndim):
 def upload_selected(coords, box, index_sets, digitized_chains=None, masses=None, device=None):
     """Move only the atoms that the call touches to the GPU: returns (coords_dev (n_used,3,F), box_dev,
     remapped index arrays, chains_dev, masses_dev).  PCIe is the end-to-end bound of this path (SURVEY 8e)."""
-    dev = _dev(device)
+    dev = _lib.device(device)
     used = np.unique(np.concatenate([np.asarray(s, dtype=np.int64).reshape(-1) for s in index_sets])) \
         if len(index_sets) else np.zeros(0, np.int64)
     if used.size and (used[0] < 0 or used[-1] >= coords.shape[0]):
@@ -303,16 +256,13 @@ def cdist(coords1, coords2, results, device=None):
     n1, n2, D = coords1.shape[0], coords2.shape[0], coords1.shape[1]
     if n1 == 0 or n2 == 0:
         return
-    dev = _dev(device)
+    dev = _lib.device(device)
     a = torch.from_numpy(np.ascontiguousarray(coords1)).to(dev)
     b = torch.from_numpy(np.ascontiguousarray(coords2)).to(dev)
     out = torch.empty((n1, n2), dtype=torch.float32, device=dev)
-    h = _lib.handle(dev.index)
-    with torch.cuda.device(dev):
-        for r0 in range(0, n1, 65535):
-            r1 = min(n1, r0 + 65535)
-            rc = _lib.load().mkb_cdist(h, _stream_ptr(dev), _ptr(a[r0:r1]), r1 - r0, _ptr(b), n2, D, _ptr(out[r0:r1]))
-            _lib.check(rc, h)
+    for r0 in range(0, n1, 65535):
+        r1 = min(n1, r0 + 65535)
+        _lib.call(dev, "mkb_cdist", _lib.ptr(a[r0:r1]), r1 - r0, _lib.ptr(b), n2, D, _lib.ptr(out[r0:r1]))
     np.copyto(results[:n1, :n2], out.cpu().numpy())
 
 
@@ -322,13 +272,10 @@ def pdist(coords, results, device=None):
     n, D = coords.shape
     if n < 2:
         return
-    dev = _dev(device)
+    dev = _lib.device(device)
     a = torch.from_numpy(np.ascontiguousarray(coords)).to(dev)
     out = torch.empty(n * (n - 1) // 2, dtype=torch.float32, device=dev)
-    h = _lib.handle(dev.index)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_pdist(h, _stream_ptr(dev), _ptr(a), n, D, _ptr(out))
-    _lib.check(rc, h)
+    _lib.call(dev, "mkb_pdist", _lib.ptr(a), n, D, _lib.ptr(out))
     np.copyto(results[:out.shape[0]], out.cpu().numpy())
 
 
@@ -339,13 +286,10 @@ def squareform(distances, device=None):
     dim = int((math.sqrt(8 * n + 1) + 1) / 2)
     if dim == 0:
         return np.zeros((0, 0), dtype=np.float32)
-    dev = _dev(device)
+    dev = _lib.device(device)
     d = torch.from_numpy(np.ascontiguousarray(distances)).to(dev)
     out = torch.empty((dim, dim), dtype=torch.float32, device=dev)
-    h = _lib.handle(dev.index)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_squareform(h, _stream_ptr(dev), _ptr(d), n, dim, _ptr(out))
-    _lib.check(rc, h)
+    _lib.call(dev, "mkb_squareform", _lib.ptr(d), n, dim, _lib.ptr(out))
     return out.cpu().numpy()
 
 
@@ -355,20 +299,11 @@ def get_collisions(coords1, coords2, dist_threshold, device=None):
     n1, n2 = coords1.shape[0], coords2.shape[0]
     if n1 == 0 or n2 == 0:
         return []
-    dev = _dev(device)
+    dev = _lib.device(device)
     a = torch.from_numpy(np.ascontiguousarray(coords1[:, :3])).to(dev)
     b = torch.from_numpy(np.ascontiguousarray(coords2[:, :3])).to(dev)
     off = torch.empty(n1 + 1, dtype=torch.int64, device=dev)
-    total = C.c_int64(0)
-    h = _lib.handle(dev.index)
-    thr = float(np.float32(dist_threshold))
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_collisions_count(h, _stream_ptr(dev), _ptr(a), n1, _ptr(b), n2, thr, _ptr(off),
-                                              C.byref(total))
-        _lib.check(rc, h)
-        pairs = torch.empty((max(total.value, 0), 2), dtype=torch.int32, device=dev)
-        if total.value > 0:
-            rc = _lib.load().mkb_collisions_fill(h, _stream_ptr(dev), _ptr(a), n1, _ptr(b), n2, thr, _ptr(off),
-                                                 _ptr(pairs))
-            _lib.check(rc, h)
+    args = (_lib.ptr(a), n1, _lib.ptr(b), n2, float(np.float32(dist_threshold)))
+    (pairs,) = _lib.count_fill(dev, "mkb_collisions_count", "mkb_collisions_fill", args, off,
+                               lambda total: (torch.empty((total, 2), dtype=torch.int32, device=dev),))
     return pairs.cpu().numpy().view(np.uint32).reshape(-1).tolist()

@@ -19,10 +19,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .align import _traj
 from .coords import _rows
-from .distance_utils import _ptr
-from .occupancy_utils import _stream_ptr
 
 LOOP, HELIX, BRIDGE, STRAND, HELIX3, HELIX5, TURN, BEND = range(8)
 LETTERS = np.array([" ", "H", "B", "E", "G", "I", "T", "S"])
@@ -78,17 +75,13 @@ def dssp_device(coords, backbone, flags, frames=None, out=None, hbonds=None):
     ``frames`` int32 (None = every frame).  ``out`` (optional) receives the (m, n) uint8 rows (unit column stride, any
     row stride).  ``hbonds`` (optional) = (partner (m, n, 2) int32, energy (m, n, 2) float64) contiguous tensors that
     receive both slots of every donor.  Returns ``out``."""
-    dev = coords.device
-    if dev.type != "cuda":
-        raise _lib.MkbError(f"dssp_device runs on CUDA tensors only, got {dev} (there is no CPU fallback)")
-    assert backbone.dtype == torch.int32 and backbone.device == dev and backbone.is_contiguous()
-    assert backbone.ndim == 2 and backbone.shape[1] == 4
+    dev = _lib.tensor_device(coords, "dssp_device")
+    _lib.index_arg(backbone, dev, cols=4)
     nres = int(backbone.shape[0])
     assert flags.dtype == torch.uint8 and flags.device == dev and flags.is_contiguous() and flags.shape == (nres,)
     if nres == 0:
         raise ValueError("dssp_device needs at least one residue")
-    if frames is not None:
-        assert frames.dtype == torch.int32 and frames.device == dev and frames.ndim == 1 and frames.is_contiguous()
+    _lib.index_arg(frames, dev)
     n = coords.shape[2] if frames is None else int(frames.numel())
     out = _rows(out, n, nres, torch.uint8, dev)
     hp = he = None
@@ -100,10 +93,7 @@ def dssp_device(coords, backbone, flags, frames=None, out=None, hbonds=None):
     if n == 0:  # an empty frame list has a NULL data pointer, which the library reads as "every frame"
         return out
     ld = max(out.stride(0) if n > 1 else nres, nres)
-    h = _lib.handle(dev.index)
-    t = _traj(coords)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_dssp(h, _stream_ptr(dev), C.byref(t), _ptr(backbone), _ptr(flags), nres,
-                                  bend_threshold(), _ptr(frames), n, _ptr(out), ld, _ptr(hp), _ptr(he))
-    _lib.check(rc, h)
+    t = _lib.traj(coords)
+    _lib.call(dev, "mkb_dssp", C.byref(t), _lib.ptr(backbone), _lib.ptr(flags), nres, bend_threshold(),
+              _lib.ptr(frames), n, _lib.ptr(out), ld, _lib.ptr(hp), _lib.ptr(he))
     return out

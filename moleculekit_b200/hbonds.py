@@ -15,8 +15,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .distance_utils import _check, _ptr, _traj, upload_selected
-from .occupancy_utils import _stream_ptr
+from .distance_utils import _check, upload_selected
 
 
 def calculate_device(coords, box, donors, acceptors, sel1, sel2, dist_threshold: float = 2.5,
@@ -26,20 +25,13 @@ def calculate_device(coords, box, donors, acceptors, sel1, sel2, dist_threshold:
     dev = coords.device
     F = coords.shape[2]
     nd, na = int(donors.shape[0]), int(acceptors.shape[0])
-    h = _lib.handle(dev.index)
-    tr = _traj(coords, box)
+    tr = _lib.traj(coords, box)
     row_off = torch.empty(F * nd + 1, dtype=torch.int64, device=dev)
-    total = C.c_int64(0)
-    args = (C.byref(tr), _ptr(donors), nd, _ptr(acceptors), na, _ptr(sel1), _ptr(sel2),
+    args = (C.byref(tr), _lib.ptr(donors), nd, _lib.ptr(acceptors), na, _lib.ptr(sel1), _lib.ptr(sel2),
             float(np.float32(dist_threshold)), float(np.float32(angle_threshold)),
             int(bool(intra)), int(bool(ignore_hs)))
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_hbonds_count(h, _stream_ptr(dev), *args, _ptr(row_off), C.byref(total))
-        _lib.check(rc, h)
-        triples = torch.empty((max(total.value, 0), 3), dtype=torch.int32, device=dev)
-        if total.value > 0:
-            rc = _lib.load().mkb_hbonds_fill(h, _stream_ptr(dev), *args, _ptr(row_off), _ptr(triples))
-            _lib.check(rc, h)
+    (triples,) = _lib.count_fill(dev, "mkb_hbonds_count", "mkb_hbonds_fill", args, row_off,
+                                 lambda total: (torch.empty((total, 3), dtype=torch.int32, device=dev),))
     frame_off = row_off[::nd] if nd > 0 else torch.zeros(F + 1, dtype=torch.int64, device=dev)
     return frame_off.contiguous(), triples
 

@@ -20,21 +20,6 @@ MAX_CHANNELS_PER_CALL = 32
 SIGMA_EXACT = 0.7
 
 
-def _dev(device) -> torch.device:
-    if device is None:
-        if not torch.cuda.is_available():
-            raise _lib.MkbError("moleculekit_b200 needs a CUDA device (there is no CPU fallback)")
-        return torch.device("cuda", torch.cuda.current_device())
-    d = torch.device(device)
-    if d.type != "cuda":
-        raise _lib.MkbError(f"moleculekit_b200 runs on CUDA devices only, got {d}")
-    return torch.device("cuda", d.index if d.index is not None else torch.cuda.current_device())
-
-
-def _stream_ptr(dev: torch.device) -> C.c_void_p:
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def make_grid_descs(origins, voxelsizes, dims, atom_offsets, out_offsets=None) -> tuple[np.ndarray, np.ndarray]:
     """Pack per-grid descriptors (``mkb_grid_desc``) for a batch.
 
@@ -143,7 +128,6 @@ def occupancy_grid_batch(coords: torch.Tensor, sigmas: torch.Tensor | None, desc
     assert coords.is_contiguous() and out.is_contiguous() and coords.ndim == 2 and coords.shape[1] == 3
     descs = np.ascontiguousarray(descs, dtype=_lib.GRID_DESC)
     flags = (_lib.OCC_ACCUMULATE if accumulate else 0) | _layout_flag(layout)
-    h = _lib.handle(dev.index)
     if sigmas is not None:
         assert sigmas.is_cuda and sigmas.device == dev and sigmas.dtype == torch.float64 and sigmas.is_contiguous()
         assert sigmas.ndim == 2 and sigmas.shape[0] == coords.shape[0]
@@ -156,18 +140,12 @@ def occupancy_grid_batch(coords: torch.Tensor, sigmas: torch.Tensor | None, desc
         Cn = int(n_channels)
     if Cn > MAX_CHANNELS_PER_CALL:
         raise ValueError(f"at most {MAX_CHANNELS_PER_CALL} channels per call; split the channel set")
-    with torch.cuda.device(dev):
-        if sigmas is not None:
-            rc = _lib.load().mkb_occupancy_grid_batch(
-                h, _stream_ptr(dev), C.c_void_p(coords.data_ptr()), C.c_void_p(sigmas.data_ptr()),
-                int(coords.shape[0]), Cn, descs.ctypes.data_as(C.c_void_p), int(descs.shape[0]),
-                C.c_void_p(out.data_ptr()), flags)
-        else:
-            rc = _lib.load().mkb_occupancy_grid_batch_masked(
-                h, _stream_ptr(dev), C.c_void_p(coords.data_ptr()), C.c_void_p(radii.data_ptr()),
-                C.c_void_p(chanmask.data_ptr()), int(coords.shape[0]), Cn, descs.ctypes.data_as(C.c_void_p),
-                int(descs.shape[0]), C.c_void_p(out.data_ptr()), flags)
-    _lib.check(rc, h)
+    if sigmas is not None:
+        _lib.call(dev, "mkb_occupancy_grid_batch", _lib.ptr(coords), _lib.ptr(sigmas), int(coords.shape[0]), Cn,
+                  descs.ctypes.data_as(C.c_void_p), int(descs.shape[0]), _lib.ptr(out), flags)
+    else:
+        _lib.call(dev, "mkb_occupancy_grid_batch_masked", _lib.ptr(coords), _lib.ptr(radii), _lib.ptr(chanmask),
+                  int(coords.shape[0]), Cn, descs.ctypes.data_as(C.c_void_p), int(descs.shape[0]), _lib.ptr(out), flags)
     return out
 
 
@@ -196,15 +174,11 @@ def occupancy_grid_batch_compact(coords: torch.Tensor, sigmas: torch.Tensor | No
         assert sigmas.is_cuda and sigmas.dtype == torch.float64 and sigmas.is_contiguous() and sigmas.shape == (coords.shape[0], 8)
     else:
         assert radii is not None and chanmask is not None and radii.dtype == torch.float64 and chanmask.dtype == torch.int32
-    h = _lib.handle(dev.index)
-    null = C.c_void_p(0)
-    with torch.cuda.device(dev):
-        rc = lib.mkb_occupancy_grid_batch_compact(
-            h, _stream_ptr(dev), C.c_void_p(coords.data_ptr()), C.c_void_p(sigmas.data_ptr()) if sigmas is not None else null,
-            C.c_void_p(radii.data_ptr()) if sigmas is None else null, C.c_void_p(chanmask.data_ptr()) if sigmas is None else null,
-            int(coords.shape[0]), descs.ctypes.data_as(C.c_void_p), int(descs.shape[0]), C.c_void_p(records.data_ptr()),
-            C.c_void_p(blk_rank.data_ptr()), int(blk_rank.numel()))
-    _lib.check(rc, h)
+    masked = sigmas is None
+    _lib.call(dev, "mkb_occupancy_grid_batch_compact", _lib.ptr(coords), _lib.ptr(sigmas),
+              _lib.ptr(radii if masked else None), _lib.ptr(chanmask if masked else None), int(coords.shape[0]),
+              descs.ctypes.data_as(C.c_void_p), int(descs.shape[0]), _lib.ptr(records), _lib.ptr(blk_rank),
+              int(blk_rank.numel()))
     return records, blk_rank
 
 
@@ -229,15 +203,11 @@ def occupancy_grid_batch_to_host(coords: torch.Tensor, sigmas: torch.Tensor | No
         assert sigmas.is_cuda and sigmas.dtype == torch.float64 and sigmas.is_contiguous() and sigmas.shape == (coords.shape[0], 8)
     else:
         assert radii is not None and chanmask is not None and radii.dtype == torch.float64 and chanmask.dtype == torch.int32
-    h = _lib.handle(dev.index)
-    null = C.c_void_p(0)
-    with torch.cuda.device(dev):
-        rc = lib.mkb_occupancy_grid_batch_to_host(
-            h, _stream_ptr(dev), C.c_void_p(coords.data_ptr()), C.c_void_p(sigmas.data_ptr()) if sigmas is not None else null,
-            C.c_void_p(radii.data_ptr()) if sigmas is None else null, C.c_void_p(chanmask.data_ptr()) if sigmas is None else null,
-            int(coords.shape[0]), descs.ctypes.data_as(C.c_void_p), int(descs.shape[0]), C.c_void_p(out_host.data_ptr()),
-            C.c_void_p(blk_rank.data_ptr()), int(blk_rank.numel()), C.c_void_p(host_rank.data_ptr()))
-    _lib.check(rc, h)
+    masked = sigmas is None
+    _lib.call(dev, "mkb_occupancy_grid_batch_to_host", _lib.ptr(coords), _lib.ptr(sigmas),
+              _lib.ptr(radii if masked else None), _lib.ptr(chanmask if masked else None), int(coords.shape[0]),
+              descs.ctypes.data_as(C.c_void_p), int(descs.shape[0]), _lib.ptr(out_host), _lib.ptr(blk_rank),
+              int(blk_rank.numel()), _lib.ptr(host_rank))
     return host_rank, blk_rank
 
 
@@ -287,15 +257,11 @@ def expand_compact_host(descs: np.ndarray, g0: int, g1: int, blk_rank: np.ndarra
 
 def grid_centers(descs: np.ndarray, device=None) -> torch.Tensor:
     """Voxel centres of a batch of grids on the device: (sum M_b, 3) float64 cuda, bit-identical to getCenters."""
-    dev = _dev(device)
+    dev = _lib.device(device)
     descs = np.ascontiguousarray(descs, dtype=_lib.GRID_DESC)
     total = int((descs["out_offset"] + descs["dims"].astype(np.int64).prod(axis=1)).max()) if len(descs) else 0
     out = torch.empty((total, 3), dtype=torch.float64, device=dev)
-    h = _lib.handle(dev.index)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_grid_centers(h, _stream_ptr(dev), descs.ctypes.data_as(C.c_void_p), int(descs.shape[0]),
-                                          C.c_void_p(out.data_ptr()))
-    _lib.check(rc, h)
+    _lib.call(dev, "mkb_grid_centers", descs.ctypes.data_as(C.c_void_p), int(descs.shape[0]), _lib.ptr(out))
     return out
 
 
@@ -310,14 +276,9 @@ def rotate_coords_device(coords: torch.Tensor, atom_offsets: torch.Tensor, matri
     B = int(atom_offsets.numel()) - 1
     assert matrices.shape == (B, 3, 3, 3) and centers.shape == (B, 3)
     out = torch.empty(coords.shape, dtype=out_dtype, device=dev)
-    p32 = C.c_void_p(out.data_ptr()) if out_dtype == torch.float32 else C.c_void_p(0)
-    p64 = C.c_void_p(out.data_ptr()) if out_dtype == torch.float64 else C.c_void_p(0)
-    h = _lib.handle(dev.index)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_rotate_coords(h, _stream_ptr(dev), C.c_void_p(coords.data_ptr()), int(coords.shape[0]),
-                                           C.c_void_p(atom_offsets.data_ptr()), B, C.c_void_p(matrices.data_ptr()),
-                                           C.c_void_p(centers.data_ptr()), p32, p64)
-    _lib.check(rc, h)
+    _lib.call(dev, "mkb_rotate_coords", _lib.ptr(coords), int(coords.shape[0]), _lib.ptr(atom_offsets), B,
+              _lib.ptr(matrices), _lib.ptr(centers), _lib.ptr(out if out_dtype == torch.float32 else None),
+              _lib.ptr(out if out_dtype == torch.float64 else None))
     return out
 
 
@@ -332,13 +293,8 @@ def occupancy_points(centers: torch.Tensor, coords: torch.Tensor, sigmas: torch.
     Cn = int(sigmas.shape[1])
     if Cn > MAX_CHANNELS_PER_CALL:
         raise ValueError(f"at most {MAX_CHANNELS_PER_CALL} channels per call; split the channel set")
-    h = _lib.handle(dev.index)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_occupancy_points(
-            h, _stream_ptr(dev), C.c_void_p(centers.data_ptr()), int(centers.shape[0]),
-            C.c_void_p(coords.data_ptr()), C.c_void_p(sigmas.data_ptr()), int(coords.shape[0]), Cn,
-            C.c_void_p(out.data_ptr()), _lib.OCC_ACCUMULATE if accumulate else 0)
-    _lib.check(rc, h)
+    _lib.call(dev, "mkb_occupancy_points", _lib.ptr(centers), int(centers.shape[0]), _lib.ptr(coords), _lib.ptr(sigmas),
+              int(coords.shape[0]), Cn, _lib.ptr(out), _lib.OCC_ACCUMULATE if accumulate else 0)
     return out
 
 
@@ -363,7 +319,7 @@ def calculate_occupancy(centers, coords, sigmas, results, device=None) -> None:
         raise ValueError("results buffer too small")
     if M == 0 or Cn == 0:
         return
-    dev = _dev(device)
+    dev = _lib.device(device)
     d_centers = torch.from_numpy(np.ascontiguousarray(centers)).to(dev)
     d_coords = torch.from_numpy(np.ascontiguousarray(coords)).to(dev)
     for c0, c1 in _channel_chunks(Cn):

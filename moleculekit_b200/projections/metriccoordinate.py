@@ -36,10 +36,10 @@ def _upload_wrap_fit(mol, centersel, pbc, refcoords, trajalnsel, refalnsel, devi
     import torch
 
     from ..align import raise_if_nonfinite, superpose_device
-    from ..occupancy_utils import _dev
+    from .. import _lib
     from ..wrapping import wrap_plan
 
-    dev = _dev(device)
+    dev = _lib.device(device)
     d = torch.from_numpy(np.ascontiguousarray(mol.coords, dtype=np.float32)).to(dev)
     if pbc:
         plan = wrap_plan(mol, centersel)

@@ -177,7 +177,7 @@ class MetricDihedral(Projection):
         import torch
 
         from ..dihedral import dihedrals_device
-        from ..occupancy_utils import _dev
+        from .. import _lib
 
         quads, _ = self._getMolProp(mol, "dihedrals")
         F, m = mol.coords.shape[2], quads.shape[0]
@@ -185,7 +185,7 @@ class MetricDihedral(Projection):
         if F == 0 or m == 0:
             return np.zeros((F, nv * m), np.float32)
         atoms, rows = np.unique(quads, return_inverse=True)
-        dev = _dev(self.device)
+        dev = _lib.device(self.device)
         d = torch.from_numpy(np.ascontiguousarray(mol.coords[atoms], dtype=np.float32)).to(dev)
         d_quads = torch.from_numpy(rows.reshape(m, 4).astype(np.int32)).to(dev)
         return dihedrals_device(d, d_quads, self._sincos).cpu().numpy()

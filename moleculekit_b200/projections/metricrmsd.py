@@ -71,7 +71,7 @@ class MetricRmsd(Projection):
         import torch
 
         from ..align import raise_if_nonfinite, rmsd_device, superpose_device
-        from ..occupancy_utils import _dev
+        from .. import _lib
         from ..wrapping import wrap_plan
 
         props = self._getMolProp(mol, "all")
@@ -83,7 +83,7 @@ class MetricRmsd(Projection):
         F = mol.coords.shape[2]
         if F == 0:
             return np.zeros(0, np.float32)
-        dev = _dev(self.device)
+        dev = _lib.device(self.device)
         d = torch.from_numpy(np.ascontiguousarray(mol.coords, dtype=np.float32)).to(dev)
         if self._pbc:
             plan = wrap_plan(mol, props["centersel"])

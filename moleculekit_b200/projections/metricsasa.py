@@ -86,14 +86,14 @@ class MetricSasa(Projection):
         """(numFrames, ncols) float32 areas in Angstrom^2."""
         import torch
 
-        from ..occupancy_utils import _dev
+        from .. import _lib
         from ..sasa import CoincidentAtomsError, sasa_device
 
         env, radii, query, groups, cols = self._getMolProp(mol, "sasa")
         F = mol.coords.shape[2]
         if F == 0:
             return np.zeros((0, len(cols)), np.float32)
-        dev = _dev(self.device)
+        dev = _lib.device(self.device)
 
         def up(a, dt):
             return torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(dev)

@@ -120,13 +120,13 @@ class MetricSecondaryStructure(Projection):
         import torch
 
         from ..dssp import dssp_device
-        from ..occupancy_utils import _dev
+        from .. import _lib
 
         backbone, flags, pos, _ = self._getMolProp(mol, "dssp")
         F, n = mol.coords.shape[2], backbone.shape[0]
         if F == 0 or n == 0:
             return self._encode(np.zeros((F, 0), np.uint8), pos)
-        dev = _dev(self.device)
+        dev = _lib.device(self.device)
         atoms, rows = np.unique(backbone, return_inverse=True)
         d = torch.from_numpy(np.ascontiguousarray(mol.coords[atoms], dtype=np.float32)).to(dev)
         d_bb = torch.from_numpy(rows.reshape(n, 4).astype(np.int32)).to(dev)

@@ -82,7 +82,7 @@ class MetricTMscore(Projection):
         """(numFrames,) float32 TM-scores."""
         import torch
 
-        from ..occupancy_utils import _dev
+        from .. import _lib
         from ..tmscore import tmscore_device
         from ..wrapping import wrap_plan
 
@@ -91,7 +91,7 @@ class MetricTMscore(Projection):
         F = mol.coords.shape[2]
         if F == 0:
             return np.zeros(0, np.float32)
-        dev = _dev(self.device)
+        dev = _lib.device(self.device)
         d = torch.from_numpy(np.ascontiguousarray(mol.coords, dtype=np.float32)).to(dev)
         if self._pbc:
             plan = wrap_plan(mol, props["centersel"])

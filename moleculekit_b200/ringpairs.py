@@ -21,8 +21,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .distance_utils import _check, _ptr, _traj, upload_selected
-from .occupancy_utils import _stream_ptr
+from .distance_utils import _check, upload_selected
 
 PIPI, CATIONPI, SIGMAHOLE = 0, 1, 2
 
@@ -34,20 +33,13 @@ def calculate_device(mode: int, coords, box, rings_atoms, starts1, second, p0, p
     F = coords.shape[2]
     n1 = int(starts1.shape[0]) - 1
     n2 = int(second.shape[0]) - 1 if mode == PIPI else int(second.shape[0])
-    h = _lib.handle(dev.index)
-    tr = _traj(coords, box)
+    tr = _lib.traj(coords, box)
     row_off = torch.empty(F * max(n1, 0) + 1, dtype=torch.int64, device=dev)
-    total = C.c_int64(0)
-    args = (int(mode), C.byref(tr), _ptr(rings_atoms), _ptr(starts1), n1, _ptr(second), n2, float(np.float32(p0)),
-            float(np.float32(p1)), float(np.float32(p2)), float(np.float32(p3)))
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_ring_pairs_count(h, _stream_ptr(dev), *args, _ptr(row_off), C.byref(total))
-        _lib.check(rc, h)
-        pairs = torch.empty((max(total.value, 0), 2), dtype=torch.int32, device=dev)
-        da = torch.empty((max(total.value, 0), 2), dtype=torch.float32, device=dev)
-        if total.value > 0:
-            rc = _lib.load().mkb_ring_pairs_fill(h, _stream_ptr(dev), *args, _ptr(row_off), _ptr(pairs), _ptr(da))
-            _lib.check(rc, h)
+    args = (int(mode), C.byref(tr), _lib.ptr(rings_atoms), _lib.ptr(starts1), n1, _lib.ptr(second), n2,
+            float(np.float32(p0)), float(np.float32(p1)), float(np.float32(p2)), float(np.float32(p3)))
+    pairs, da = _lib.count_fill(dev, "mkb_ring_pairs_count", "mkb_ring_pairs_fill", args, row_off,
+                                lambda total: (torch.empty((total, 2), dtype=torch.int32, device=dev),
+                                               torch.empty((total, 2), dtype=torch.float32, device=dev)))
     frame_off = row_off[::n1] if n1 > 0 else torch.zeros(F + 1, dtype=torch.int64, device=dev)
     return frame_off.contiguous(), pairs, da
 

@@ -15,10 +15,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .align import _traj
 from .coords import _rows
-from .distance_utils import _ptr
-from .occupancy_utils import _stream_ptr
 
 MAX_SPHERE_POINTS = 65536
 
@@ -102,16 +99,14 @@ def sasa_device(coords, env, radii, query, sphere, groups=None, frames=None, out
     offsets into ``query``: column g is then the float32 sum, in order, of the areas of query[groups[g]:groups[g+1]].
     ``frames`` int32 (None = every frame).  ``out`` (optional) receives the rows (unit column stride, any row stride).
     Raises :class:`CoincidentAtomsError` when a query atom coincides with another ``env`` atom."""
-    dev = coords.device
-    if dev.type != "cuda":
-        raise _lib.MkbError(f"sasa_device runs on CUDA tensors only, got {dev} (there is no CPU fallback)")
-    for t, dt in ((env, torch.int32), (radii, torch.float32), (query, torch.int32), (sphere, torch.float32)):
-        assert t.dtype == dt and t.device == dev and t.is_contiguous()
-    assert env.ndim == 1 and radii.shape == env.shape and query.ndim == 1 and sphere.ndim == 2 and sphere.shape[1] == 3
-    if groups is not None:
-        assert groups.dtype == torch.int64 and groups.device == dev and groups.ndim == 1 and groups.is_contiguous()
-    if frames is not None:
-        assert frames.dtype == torch.int32 and frames.device == dev and frames.ndim == 1 and frames.is_contiguous()
+    dev = _lib.tensor_device(coords, "sasa_device")
+    _lib.index_arg(env, dev)
+    _lib.index_arg(query, dev)
+    _lib.index_arg(groups, dev, torch.int64)
+    _lib.index_arg(frames, dev)
+    for t in (radii, sphere):
+        assert t.dtype == torch.float32 and t.device == dev and t.is_contiguous()
+    assert radii.shape == env.shape and sphere.ndim == 2 and sphere.shape[1] == 3
     cols = int(query.numel()) if groups is None else int(groups.numel()) - 1
     n = coords.shape[2] if frames is None else int(frames.numel())
     out = _rows(out, n, cols, torch.float32, dev)
@@ -119,13 +114,10 @@ def sasa_device(coords, env, radii, query, sphere, groups=None, frames=None, out
         return out
     ld = max(out.stride(0) if n > 1 else cols, cols)
     status = torch.empty(1, dtype=torch.int64, device=dev)
-    h = _lib.handle(dev.index)
-    t = _traj(coords)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_sasa(h, _stream_ptr(dev), C.byref(t), _ptr(env), int(env.numel()), _ptr(radii),
-                                  _ptr(query), int(query.numel()), _ptr(groups), max(cols, 0) if groups is not None else 0,
-                                  _ptr(sphere), int(sphere.shape[0]), _ptr(frames), n, _ptr(out), ld, _ptr(status))
-    _lib.check(rc, h)
+    t = _lib.traj(coords)
+    _lib.call(dev, "mkb_sasa", C.byref(t), _lib.ptr(env), int(env.numel()), _lib.ptr(radii), _lib.ptr(query),
+              int(query.numel()), _lib.ptr(groups), max(cols, 0) if groups is not None else 0, _lib.ptr(sphere),
+              int(sphere.shape[0]), _lib.ptr(frames), n, _lib.ptr(out), ld, _lib.ptr(status))
     key = int(status.item())
     if key != -1:
         _raise_coincident(coords, env, query, frames, key)

@@ -19,9 +19,6 @@ import numpy as np
 import torch
 
 from . import _lib
-from .align import _traj
-from .distance_utils import _ptr
-from .occupancy_utils import _dev, _stream_ptr
 
 
 def tm_parameters(L: int, lnorm: int):
@@ -66,9 +63,7 @@ def tmscore_device(coords, sel, refcoords, refsel, frames=None):
     (M, 3, 1).  ``sel`` (n,) and ``refsel`` (m,) int32 CUDA tensors are the paired atoms in pairing order: L = min(n, m)
     pairs, normalised by m.  ``frames`` int32 (None = every frame).  Returns (tm (len,) float64, rmsd (len,) float64);
     a frame with a non-finite paired coordinate gets NaN for both."""
-    dev = coords.device
-    if dev.type != "cuda":
-        raise _lib.MkbError(f"tmscore_device runs on CUDA tensors only, got {dev} (there is no CPU fallback)")
+    dev = _lib.tensor_device(coords, "tmscore_device")
     n, m = int(sel.numel()), int(refsel.numel())
     if n == 0 or m == 0:
         raise RuntimeError(f"TM-score selections resulted in {n} and {m} atoms.")
@@ -76,8 +71,8 @@ def tmscore_device(coords, sel, refcoords, refsel, frames=None):
     cap = max_pairs()
     if L > cap:
         raise ValueError(f"TM-score over {L} pairs: at most {cap} pairs fit one call")
-    for t in (sel, refsel) + (() if frames is None else (frames,)):
-        assert t.dtype == torch.int32 and t.device == dev and t.ndim == 1 and t.is_contiguous()
+    for x in (sel, refsel, frames):
+        _lib.index_arg(x, dev)
     if not bool(torch.isfinite(refcoords[refsel[:L].long(), :, 0]).all()):
         raise ValueError("the reference has non-finite coordinates among the paired atoms")
     d0, d0s, frag = tm_parameters(L, m)
@@ -87,13 +82,9 @@ def tmscore_device(coords, sel, refcoords, refsel, frames=None):
     rmsd = torch.empty(cnt, dtype=torch.float64, device=dev)
     if cnt == 0:  # an empty frame list has a NULL data pointer, which the library reads as "every frame"
         return tm, rmsd
-    h = _lib.handle(dev.index)
-    t, r = _traj(coords), _traj(refcoords)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_tmscore(h, _stream_ptr(dev), C.byref(t), _ptr(sel), C.byref(r), _ptr(refsel), L, m, d0, d0s,
-                                     frag.ctypes.data_as(C.c_void_p), int(frag.size), _ptr(frames), cnt, _ptr(tm),
-                                     _ptr(rmsd))
-    _lib.check(rc, h)
+    t, r = _lib.traj(coords), _lib.traj(refcoords)
+    _lib.call(dev, "mkb_tmscore", C.byref(t), _lib.ptr(sel), C.byref(r), _lib.ptr(refsel), L, m, d0, d0s,
+              frag.ctypes.data_as(C.c_void_p), int(frag.size), _lib.ptr(frames), cnt, _lib.ptr(tm), _lib.ptr(rmsd))
     return tm, rmsd
 
 
@@ -107,7 +98,7 @@ def molTMscore(mol, ref, selCAmol, selCAref, device=None):
     F = mol.coords.shape[2]
     if F == 0:
         return np.zeros(0), np.zeros(0), np.zeros(0, np.int64)
-    dev = _dev(device)
+    dev = _lib.device(device)
     x = torch.from_numpy(np.ascontiguousarray(mol.coords[idx[:L]], dtype=np.float32)).to(dev)
     fr = int(getattr(ref, "frame", 0))
     y = torch.from_numpy(np.ascontiguousarray(ref.coords[ridx][:, :, fr:fr + 1], dtype=np.float32)).to(dev)

@@ -138,7 +138,7 @@ def rotateCoordinates(coords: np.ndarray, rotations: list, center: list, device=
         raise ValueError("coords must have shape (natoms, 3)")
     if not np.array_equal(c32, np.asarray(coords)):
         raise ValueError("rotateCoordinates on the GPU takes float32-representable coordinates (Molecule.coords)")
-    dev = _occ._dev(device)
+    dev = _lib_mod.device(device)
     d = _occ.rotate_coords_device(torch.from_numpy(c32).to(dev),
                                   torch.tensor([0, c32.shape[0]], dtype=torch.int64, device=dev),
                                   torch.from_numpy(rotation_matrices(list(rotations))).to(dev),
@@ -175,7 +175,7 @@ def _occupancy_grid(coords, sigmas, bb_min, nvoxels, voxelsize, device=None) -> 
     """One regular grid -> (M, C) float64 numpy (the `_getOccupancyC` of the reference, :515-533)."""
     coords = np.ascontiguousarray(np.asarray(coords).astype(np.float32))
     sigmas = np.ascontiguousarray(np.asarray(sigmas).astype(np.float64))
-    dev = _occ._dev(device)
+    dev = _lib_mod.device(device)
     M = int(np.prod(nvoxels))
     Cn = sigmas.shape[1]
     feats = np.empty((M, Cn), dtype=np.float64)
@@ -336,7 +336,7 @@ class VoxelBatch:
 
     def to_device(self, device=None):
         """(coords, channels) on the device; channels = the sigma matrix, or the (radii, bit mask) pair."""
-        dev = _occ._dev(device)
+        dev = _lib_mod.device(device)
         d_coords = torch.from_numpy(self.coords).to(dev, non_blocking=True)
         if self.sigmas is not None:
             return d_coords, torch.from_numpy(self.sigmas).to(dev, non_blocking=True)
@@ -505,7 +505,7 @@ def getVoxelDescriptorsBatch(coords, channels, *, boxsize=None, centers=None, bu
     float64 -- with identical bytes; "auto" takes the compact route when it applies."""
     batch = VoxelBatch(coords, channels, boxsize=boxsize, centers=centers, buffer=buffer, voxelsize=voxelsize,
                        elements=elements, radii=radii, atom_offsets=atom_offsets)
-    dev = _occ._dev(device)
+    dev = _lib_mod.device(device)
     d_coords, d_chan = batch.to_device(dev)
     if rotations is not None:
         if rotation_centers is None:

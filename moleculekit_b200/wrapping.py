@@ -24,8 +24,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .distance_utils import _check, _ptr, _traj
-from .occupancy_utils import _dev, _stream_ptr
+from .distance_utils import _check
 
 logger = logging.getLogger(__name__)
 
@@ -38,14 +37,9 @@ def wrap_box_device(coords: torch.Tensor, box: torch.Tensor, groups: torch.Tenso
     dev = coords.device
     ncs = 0 if centersel is None else int(centersel.numel())
     cen = (C.c_float * 3)(*([0.0, 0.0, 0.0] if center is None else [float(np.float32(c)) for c in center]))
-    if coords.shape[2] <= 1 and not coords.is_contiguous():
-        raise ValueError("coords must be contiguous for in-place wrapping")
-    h = _lib.handle(dev.index)
-    tr = _traj(coords, box)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_wrap_box(h, _stream_ptr(dev), C.byref(tr), _ptr(groups), int(groups.numel()),
-                                      _ptr(centersel) if ncs else C.c_void_p(0), ncs, cen)
-    _lib.check(rc, h)
+    tr = _lib.traj(coords, box, writable=True)
+    _lib.call(dev, "mkb_wrap_box", C.byref(tr), _lib.ptr(groups), int(groups.numel()),
+              _lib.ptr(centersel if ncs else None), ncs, cen)
     return coords
 
 
@@ -69,14 +63,14 @@ def wrap_triclinic_device(coords: torch.Tensor, boxvectors: torch.Tensor, groups
     else:
         assert boxvectors.stride(2) == 1 and boxvectors.stride(0) == 3 * boxvectors.stride(1)
         bvs = boxvectors.stride(1)
-    h = _lib.handle(dev.index)
-    tr = _traj(coords, torch.zeros((3, max(F, 1)), dtype=torch.float32, device=dev)[:, :F])
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_wrap_triclinic(h, _stream_ptr(dev), C.byref(tr), _ptr(boxvectors), int(bvs), _ptr(groups),
-                                            int(groups.numel()), _ptr(centersel) if ncs else C.c_void_p(0), ncs, cen, mode)
-    if rc != 0 and b"Too many triclinic vectors" in (_lib.load().mkb_last_error(h) or b""):
-        raise ValueError("Too many triclinic vectors!!")  # wrapping.pyx:439-441
-    _lib.check(rc, h)
+    tr = _lib.traj(coords, writable=True)
+    try:
+        _lib.call(dev, "mkb_wrap_triclinic", C.byref(tr), _lib.ptr(boxvectors), int(bvs), _lib.ptr(groups),
+                  int(groups.numel()), _lib.ptr(centersel if ncs else None), ncs, cen, mode)
+    except _lib.MkbError as e:
+        if "Too many triclinic vectors" in str(e):
+            raise ValueError("Too many triclinic vectors!!") from None  # wrapping.pyx:439-441
+        raise
     return coords
 
 
@@ -115,7 +109,7 @@ def _run_host(plan, coords, box, device):
     if plan.is_noop(coords.shape[0], coords.shape[2]):
         return
     _check_index_ranges(plan.groups, plan.centersel, coords.shape[0])  # bad input is rejected before any device work
-    dev = _dev(device)
+    dev = _lib.device(device)
     d_coords = torch.from_numpy(np.ascontiguousarray(coords)).to(dev)
     d_box = None if box is None else torch.from_numpy(np.ascontiguousarray(box, dtype=np.float32)).to(dev)
     plan.run_device(d_coords, d_box)

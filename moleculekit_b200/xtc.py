@@ -15,7 +15,6 @@ import numpy as np
 import torch
 
 from . import _lib
-from .occupancy_utils import _dev, _stream_ptr
 
 XTC_MAGIC = 1995
 # numpy mirror of `mkb_xtc_frame` (48 bytes)
@@ -81,12 +80,8 @@ def decode_xtc_device(file_bytes: torch.Tensor, frames: np.ndarray, natoms: int,
         out = torch.empty((natoms, 3, F), dtype=torch.float32, device=dev)
     assert out.shape == (natoms, 3, F) and out.dtype == torch.float32 and out.is_contiguous()
     status = torch.zeros(max(F, 1), dtype=torch.int32, device=dev)
-    h = _lib.handle(dev.index)
-    with torch.cuda.device(dev):
-        rc = _lib.load().mkb_xtc_decode(h, _stream_ptr(dev), C.c_void_p(file_bytes.data_ptr()), int(file_bytes.numel()),
-                                        frames.ctypes.data_as(C.c_void_p), F, int(natoms), C.c_void_p(out.data_ptr()),
-                                        max(F, 1), float(scale), C.c_void_p(status.data_ptr()))
-    _lib.check(rc, h)
+    _lib.call(dev, "mkb_xtc_decode", _lib.ptr(file_bytes), int(file_bytes.numel()), frames.ctypes.data_as(C.c_void_p), F,
+              int(natoms), _lib.ptr(out), max(F, 1), float(scale), _lib.ptr(status))
     bad = torch.nonzero(status[:F]).flatten()
     if bad.numel():
         raise RuntimeError(f"Malformed XTC file: frame {int(bad[0])} could not be decoded (status {int(status[bad[0]])})")
@@ -106,7 +101,7 @@ def read_xtc_device(filename, frames=None, scale: float = 1.0, device=None):
     raw = _load(filename)
     idx = index_xtc(raw)
     sel = slice(None) if frames is None else np.asarray(frames, dtype=np.int64)
-    dev = _dev(device)
+    dev = _lib.device(device)
     # (+4 zero bytes: the kernel reads whole 32-bit words, and a file cut right after its last block has no XDR padding)
     d_bytes = torch.frombuffer(bytearray(raw) + bytearray(4), dtype=torch.uint8).to(dev)
     coords = decode_xtc_device(d_bytes, idx["frames"][sel], idx["natoms"], scale=scale)
