@@ -32,7 +32,7 @@ enum ScratchSlot {
     S_QUEUE,        // occupancy run kernel: block queue counter
     S_FIX_LIST,     // occupancy run kernel: voxels re-evaluated in float64 (count + list)
     S_BLK_ENT,      // occupancy run kernel: per-block candidate lists
-    S_BLK_SLOTS,    // occupancy run kernel: the slot of every (atom, block) insertion
+    S_BLK_SEGS,     // occupancy run kernel: the (CTA, block) list segments reserved by the count pass
     S_ALIGN_PART,   // K14: per-(segment, frame) partial sums of the fit / RMSD
     S_ALIGN_REF,    // K14: the centred reference selection
     S_COORD_PART,   // K15: per-(frame chunk, atom, axis) partial frame sums

@@ -5,8 +5,8 @@
 // flush, FFMA.SAT gate ...) are in the git history of this file together with their compile-time selectors.
 //
 //   * K2' (occ_prep_kernel / occ_blk_fill_kernel): every atom is appended to the candidate list of each 4x4x8-voxel
-//     block it can reach (~16 blocks per atom at 1 A) -- count, scan, fill, both walks counting per CTA and block in
-//     shared memory.  The fill kernel reads its list; no block scans cell rows.
+//     block it can reach (~16 blocks per atom at 1 A) -- count (per CTA and block in shared memory, reserving the CTA's
+//     list segments), scan, fill (one walk).  The fill kernel reads its list; no block scans cell rows.
 //   * value = max_a [d2 < cut2] f(sigma^2 / d2) with f monotone: the kernel tracks  r = d2 / sigma^2  as a MIN and applies f
 //     once per voxel-channel; no reciprocal per pair.
 //   * One warp owns a block; a lane owns the 4 voxels of one x-row (they share dy, dz).  The candidate is WARP-UNIFORM (two
@@ -109,13 +109,18 @@ __device__ __forceinline__ void for_each_block_in_reach(const GridDev &g, float 
     }
 }
 
-// The atoms of one CTA share most of their blocks (C3: ~4 200 insertions into ~700 blocks per 256 atoms), so both list
-// passes count per (CTA, block) in a shared-memory hash table keyed by the global block slot (tile_base + block id; a CTA
-// may span several grids; linear probing) and touch global memory once per occupied entry.  An insertion whose key finds
-// neither itself nor a free slot within L_PROBES slots goes to global memory directly.  Keys are never removed, so every
-// insertion of a key within a CTA takes the same route in both walks of the fill pass.  At fine voxel sizes the atoms
-// of a CTA reach far more blocks than the table holds (C5, 0.5 A: ~100 blocks per atom, ~9 000 per CTA); there the
-// host turns the table off (`table` = 0) and every insertion takes the direct route.
+// The atoms of one CTA share most of their blocks (C3: ~4 200 insertions into ~700 blocks per 256 atoms), so the count
+// pass counts per (CTA, block) in a shared-memory hash table keyed by the global block slot (tile_base + block id; a CTA
+// may span several grids; linear probing) and touches global memory once per occupied entry.  An insertion whose key
+// finds neither itself nor a free slot within L_PROBES slots is counted in global memory directly (blk_direct).  Keys
+// are never removed, so within a CTA a key is either entirely in the table or entirely direct, and a table rebuilt with
+// every key at its slot routes each insertion as the count pass did.  At fine voxel sizes the atoms of a CTA reach far
+// more blocks than the table holds (C5, 0.5 A: ~100 blocks per atom, ~9 000 per CTA); there the host turns the table off
+// (`table` = 0) and every insertion takes the direct route.
+//
+// The list of block k spans [blk_start[k], blk_start[k + 1]) = blk_count[k] in-table entries + blk_direct[k] direct ones.
+// The direct entries fill it from the front, the in-table segments from the back: the count pass's
+// atomicAdd(blk_count + k, n) returns the CTA's segment base b, and the segment is [blk_start[k + 1] - b - n, .. - b).
 constexpr int L_THREADS = 256;          // atoms per CTA of the two list passes
 constexpr int L_TABLE = 2048;           // hash slots per CTA (power of two)
 constexpr int L_PROBES = 8;             // linear-probing limit
@@ -123,7 +128,14 @@ constexpr int L_STAGE = 4096;           // entries per CTA staged in shared memo
 constexpr int L_TABLE_MAX_REACH = 64;   // the host uses the table when an atom reaches at most this many blocks
 constexpr unsigned L_EMPTY = 0xffffffffu;
 constexpr int L_SLOTS = L_TABLE / L_THREADS;  // slots per thread in the fill pass's scan
+constexpr int L_SEG_WORDS = 3 * L_TABLE;      // per CTA: the keys, segment bases and slot | n << 11 of its occupied slots
 static_assert(L_TABLE <= 2048 && L_THREADS <= 256, "a staged entry packs slot (11 bits) | thread (8) | mask (9)");
+
+// scan input: the length of block i's list
+struct ListLength {
+    const unsigned *count, *direct;
+    __host__ __device__ unsigned operator()(int i) const { return count[i] + direct[i]; }
+};
 
 __device__ __forceinline__ unsigned list_hash(unsigned key) { return (key * 2654435761u) >> (32 - 11); }
 static_assert(L_TABLE == 1 << 11, "list_hash yields 11 bits");
@@ -157,7 +169,7 @@ __device__ __forceinline__ void list_table_clear(unsigned *s_key, unsigned *s_cn
 __device__ __forceinline__ void occ_prep_item(const float *__restrict__ coords, const double *__restrict__ sigmas,
                                               const double *__restrict__ radii, const unsigned *__restrict__ chanmask,
                                               const GridDev *__restrict__ grids, int B, long long it, float4 *__restrict__ rec_pos,
-                                              uint4 *__restrict__ rec_tag, unsigned *__restrict__ blk_count, int table,
+                                              uint4 *__restrict__ rec_tag, unsigned *__restrict__ blk_direct, int table,
                                               unsigned *s_key, unsigned *s_cnt) {
     const int b = find_grid_item(grids, B, it);
     const GridDev &g = grids[b];
@@ -203,40 +215,74 @@ __device__ __forceinline__ void occ_prep_item(const float *__restrict__ coords, 
     for_each_block_in_reach(g, (float)ip[0] + f[0], (float)ip[1] + f[1], (float)ip[2] + f[2], [&](int bid) {
         const int s = table ? list_slot_insert(s_key, tb + bid) : -1;
         if (s >= 0) atomicAdd(s_cnt + s, 1u);
-        else atomicAdd(blk_count + tb + bid, 1u);
+        else atomicAdd(blk_direct + tb + bid, 1u);
     });
 }
 
+// count pass: records, then per occupied table slot one atomicAdd reserves the CTA's segment of that block's list; with
+// the table on, the CTA keeps (key, base, slot | n << 11) of every occupied slot, compacted, in its L_SEG_WORDS of `segs`
+// and their number in seg_n[CTA] for the fill pass.
 __global__ void __launch_bounds__(L_THREADS) occ_prep_kernel(const float *__restrict__ coords, const double *__restrict__ sigmas,
                                                              const double *__restrict__ radii, const unsigned *__restrict__ chanmask,
                                                              const GridDev *__restrict__ grids, int B, long long n_items,
                                                              float4 *__restrict__ rec_pos, uint4 *__restrict__ rec_tag,
-                                                             unsigned *__restrict__ blk_count, int table) {
-    __shared__ unsigned s_key[L_TABLE], s_cnt[L_TABLE];
+                                                             unsigned *__restrict__ blk_count, unsigned *__restrict__ blk_direct,
+                                                             unsigned *__restrict__ segs, unsigned *__restrict__ seg_n, int table) {
+    __shared__ unsigned s_key[L_TABLE], s_cnt[L_TABLE], s_nseg;
     list_table_clear(s_key, s_cnt);
+    if (threadIdx.x == 0) s_nseg = 0u;
     __syncthreads();
     const long long it = blockIdx.x * (long long)L_THREADS + threadIdx.x;
-    if (it < n_items) occ_prep_item(coords, sigmas, radii, chanmask, grids, B, it, rec_pos, rec_tag, blk_count, table, s_key, s_cnt);
+    if (it < n_items) occ_prep_item(coords, sigmas, radii, chanmask, grids, B, it, rec_pos, rec_tag, blk_direct, table, s_key, s_cnt);
+    if (!table) return;
     __syncthreads();
-    for (int i = threadIdx.x; i < L_TABLE; i += L_THREADS)
-        if (s_key[i] != L_EMPTY) atomicAdd(blk_count + s_key[i], s_cnt[i]);
+    unsigned *const seg = segs + (size_t)blockIdx.x * L_SEG_WORDS;
+    const unsigned lane = threadIdx.x & 31u;
+#pragma unroll
+    for (int i = threadIdx.x; i < L_TABLE; i += L_THREADS) {  // warp-uniform trip count
+        const unsigned key = s_key[i];
+        const unsigned occ = __ballot_sync(0xffffffffu, key != L_EMPTY);
+        unsigned j0 = 0;
+        if (lane == 0 && occ) j0 = atomicAdd(&s_nseg, (unsigned)__popc(occ));
+        j0 = __shfl_sync(0xffffffffu, j0, 0);
+        if (key != L_EMPTY) {
+            const unsigned n = s_cnt[i], j = j0 + __popc(occ & ((1u << lane) - 1u));
+            seg[j] = key;
+            seg[L_TABLE + j] = atomicAdd(blk_count + key, n);
+            seg[2 * L_TABLE + j] = (unsigned)i | n << 11;
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) seg_n[blockIdx.x] = s_nseg;
 }
 
-// second pass: the same walk appends (item, mask | multi << 8) to the lists; blk_count counts down to zero.  Walk 1 counts
-// the CTA's insertions per block in the table, one atomicSub per occupied entry reserves the segment [old - n, old) of
-// that block's list, and walk 2 places every insertion at its segment's base + a shared cursor.  The first L_STAGE
-// entries of the CTA are staged in shared memory in segment order (one word: table slot, thread, mask) and leave in one
-// pass at the end, consecutive threads writing consecutive list positions (one scattered 8-byte store per entry took
-// most of the pass); entries beyond L_STAGE are stored at once.  Insertions outside the table reserve and store their
-// entry one by one.  (Keeping the slots of the first pass instead was slower.)
+// fill pass: the same walk appends (item, mask | multi << 8) to the lists.  The CTA puts the count pass's occupied slots
+// back at their slot indices (the same slots, so list_slot_find routes every insertion as the count pass did) and one walk
+// places each in-table insertion at its segment's start + a shared cursor.  The first L_STAGE entries of the CTA are
+// staged in shared memory in segment order (one word: table slot, thread, mask) and leave in one pass at the end,
+// consecutive threads writing consecutive list positions (one scattered 8-byte store per entry took most of the pass);
+// entries beyond L_STAGE are stored at once.  Direct insertions take their position one by one from blk_direct, which
+// counts down to zero.
 __global__ void __launch_bounds__(L_THREADS, 5) occ_blk_fill_kernel(const GridDev *__restrict__ grids, int B, long long n_items,
                                                                  const float4 *__restrict__ rec_pos, const uint4 *__restrict__ rec_tag,
-                                                                 unsigned *__restrict__ blk_count, const unsigned *__restrict__ blk_start,
+                                                                 unsigned *__restrict__ blk_direct, const unsigned *__restrict__ blk_start,
+                                                                 const unsigned *__restrict__ segs, const unsigned *__restrict__ seg_n,
                                                                  uint2 *__restrict__ blk_ent, int table) {
     // keys, cursors, list position - staged index per slot; staged entries; warp sums of the scan
     __shared__ unsigned s_key[L_TABLE], s_cur[L_TABLE], s_off[L_TABLE], s_stage[L_STAGE], s_wsum[L_THREADS / 32];
     list_table_clear(s_key, s_cur);
     __syncthreads();
+    if (table) {
+        const unsigned *const seg = segs + (size_t)blockIdx.x * L_SEG_WORDS;
+        const unsigned ns = seg_n[blockIdx.x];
+        for (unsigned j = threadIdx.x; j < ns; j += L_THREADS) {
+            const unsigned key = seg[j], base = seg[L_TABLE + j], sn = seg[2 * L_TABLE + j];
+            const unsigned s = sn & (L_TABLE - 1), n = sn >> 11;
+            s_key[s] = key;
+            s_cur[s] = n;
+            s_off[s] = blk_start[key + 1] - base - n;  // segment start; the staged index is subtracted below
+        }
+    }
     const long long it = blockIdx.x * (long long)L_THREADS + threadIdx.x;
     uint4 tg = make_uint4(0u, 0u, 0u, 0u);
     if (it < n_items) tg = rec_tag[it];
@@ -250,12 +296,6 @@ __global__ void __launch_bounds__(L_THREADS, 5) occ_blk_fill_kernel(const GridDe
         px = (float)((int)(tg.z & 0xffffu) - off) + f.x;
         py = (float)((int)(tg.z >> 16) - off) + f.y;
         pz = (float)((int)(tg.x >> 16) - off) + f.z;
-        const unsigned tb = (unsigned)g->tile_base;
-        if (table)  // without the table walk 2 finds every key absent
-            for_each_block_in_reach(*g, px, py, pz, [&](int bid) {
-                const int s = list_slot_insert(s_key, tb + bid);
-                if (s >= 0) atomicAdd(s_cur + s, 1u);
-            });
     }
     __syncthreads();
     // segments in slot order: thread t scans L_SLOTS consecutive slots, the staged order is an exclusive scan of the counts
@@ -281,9 +321,8 @@ __global__ void __launch_bounds__(L_THREADS, 5) occ_blk_fill_kernel(const GridDe
 #pragma unroll
     for (int j = 0; j < L_SLOTS; ++j) {
         const int i = threadIdx.x * L_SLOTS + j;
-        const unsigned key = s_key[i];
-        if (key != L_EMPTY) {
-            s_off[i] = blk_start[key] + atomicSub(blk_count + key, n[j]) - n[j] - loff;  // list position - staged index
+        if (s_key[i] != L_EMPTY) {
+            s_off[i] -= loff;  // list position - staged index
             s_cur[i] = loff;
         }
         loff += n[j];
@@ -300,7 +339,7 @@ __global__ void __launch_bounds__(L_THREADS, 5) occ_blk_fill_kernel(const GridDe
                 if (li < (unsigned)L_STAGE) s_stage[li] = (unsigned)s << 17 | threadIdx.x << 9 | ent.y;
                 else blk_ent[s_off[s] + li] = ent;
             } else {
-                blk_ent[blk_start[key] + atomicSub(blk_count + key, 1u) - 1u] = ent;
+                blk_ent[blk_start[key] + atomicSub(blk_direct + key, 1u) - 1u] = ent;
             }
         });
     }
@@ -763,6 +802,13 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
 constexpr float R_FIND_BAND = 2.0e-6f;  // relative; fill error (< 1e-6, see DESIGN.md) + this kernel's own float32 error
 constexpr int FIX_HDR = 4;              // words in front of the list: count
 
+// MUFU.SQRT (relative error ~2^-22) for the loop bounds, which carry their own slack; sqrtf would add the IEEE slow path
+__device__ __forceinline__ float sqrt_bound(float x) {
+    float r;
+    asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
+    return r;
+}
+
 __global__ void __launch_bounds__(128) occ_band_kernel(const float *__restrict__ coords, const GridDev *__restrict__ grids, int B,
                                                        long long n_items, unsigned *__restrict__ bitmap,
                                                        unsigned long long *__restrict__ fix, unsigned cap) {
@@ -785,42 +831,64 @@ __global__ void __launch_bounds__(128) occ_band_kernel(const float *__restrict__
     if (!live) return;  // NaN or out of reach of every voxel
     const float cut2 = g.cut2v;
     const float band = R_FIND_BAND * cut2;
-    const int W = (int)(sqrtf(cut2) + 0.5f) + 1;  // |j - f| <= cut with |f| <= 0.5 (+1: rounding slack)
+    const int W = (int)(sqrt_bound(cut2) + 0.5f) + 1;  // |j - f| <= cut with |f| <= 0.5 (+1: rounding slack)
     const float RND = 12582912.0f;                  // 1.5 * 2^23: (x + RND) - RND == rint(x) for |x| < 2^22
-    const int ny = g.dims[1], nz = g.dims[2];
-    for (int jy = -W; jy <= W; ++jy) {
+    const int nx = g.dims[0], ny = g.dims[1], nz = g.dims[2];
+    // rows outside the grid flag nothing: the y and z ranges stop at its faces
+    const int jy_lo = max(-W, -ip[1]), jy_hi = min(W, ny - 1 - ip[1]);
+    int jz_min = max(-W, -ip[2]);
+    const int jz_max = min(W, nz - 1 - ip[2]);
+    // ptxas (CUDA 12.9, sm_90a) folds max(max(-W, -ip), c) into one three-input VIMNMX3 and loses the negation of ip; the
+    // opaque move keeps jz_min a register of its own
+    asm("mov.b32 %0, %0;" : "+r"(jz_min));
+    for (int jy = jy_lo; jy <= jy_hi; ++jy) {
         const int iy = ip[1] + jy;
         const float dy = (float)jy - f[1];
         const float A = fmaf(-dy, dy, cut2);
-        if (A < -band || iy < 0 || iy >= ny) continue;
-        // z rows that can cross the sphere: |jz - f_z| <= sqrt(A + band) (a superset; the exact test follows per row)
-        const float zr = sqrtf(A + band) + 1e-3f;
-        const int jz_lo = max(-W, (int)ceilf(f[2] - zr)), jz_hi = min(W, (int)floorf(f[2] + zr));
+        if (A < -band) continue;
+        // z rows that can cross the sphere: |jz - f_z| <= sqrt(A + band) (a superset: the 1e-3 margin covers the approximate
+        // square root, and the exact test follows per row)
+        const float zr = sqrt_bound(A + band) + 1e-3f;
+        const int jz_lo = max(jz_min, (int)ceilf(f[2] - zr)), jz_hi = min(jz_max, (int)floorf(f[2] + zr));
+        // The row loop only searches: it leaves at the last row or at a row that flags a voxel, which is handled outside it
+        // (rare: ~10 voxels per pocket), and resumes after it -- no reconvergence point per row.  A row that misses the
+        // sphere (h2 < -band) has hh = 0, so jxb == jxa and ta >= -h2 > band: it flags nothing without a test of its own.
+        // (A float row counter would save the I2FP, but ptxas then puts a YIELD in the row loop: the kernel took twice as
+        // long on an H100.)
         for (int jz = jz_lo; jz <= jz_hi; ++jz) {
-            const float dz = (float)jz - f[2];
-            const float h2 = fmaf(-dz, dz, A);  // cut2 - s
-            if (h2 < -band) continue;           // the row misses the sphere
-            const float hp = fmaxf(h2, 0.0f);
-            const float hh = hp * rsqrtf(fmaxf(hp, 1e-30f));
-            const float jxa = (f[0] + hh + RND) - RND, jxb = (f[0] - hh + RND) - RND;
-            const float da = jxa - f[0], db = jxb - f[0];
-            const float ta = fmaf(da, da, -h2), tb = fmaf(db, db, -h2);
+            float h2, jxa, jxb, ta, tb;
+            bool hit;
+            for (;; ++jz) {
+                const float dz = (float)jz - f[2];
+                h2 = fmaf(-dz, dz, A);  // cut2 - s
+                const float hp = fmaxf(h2, 0.0f);
+                // rsqrt of a normal number: the FTZ form is the same instruction without the denormal guard, and for
+                // hp < FLT_MIN, hh < 2^-63 leaves the roundings below unchanged
+                float rs;
+                asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(rs) : "f"(fmaxf(hp, FLT_MIN)));
+                const float hh = hp * rs;
+                jxa = (f[0] + hh + RND) - RND;
+                jxb = (f[0] - hh + RND) - RND;
+                const float da = jxa - f[0], db = jxb - f[0];
+                ta = fmaf(da, da, -h2);
+                tb = fmaf(db, db, -h2);
+                hit = (fabsf(ta) <= band) | ((fabsf(tb) <= band) & (jxb != jxa));
+                if (hit | (jz >= jz_hi)) break;
+            }
+            if (!hit) break;
             const bool fa = fabsf(ta) <= band, fb = (fabsf(tb) <= band) & (jxb != jxa);
-            if (fa | fb) {
-                const int iz = ip[2] + jz;
-                if (iz < 0 || iz >= nz) continue;
+            const unsigned iz = (unsigned)(ip[2] + jz);  // in [0, nz)
 #pragma unroll
-                for (int q = 0; q < 2; ++q) {
-                    if (q == 0 ? !fa : !fb) continue;
-                    const int ix = ip[0] + (int)(q == 0 ? jxa : jxb);
-                    if (ix < 0 || ix >= g.dims[0]) continue;
-                    const long long v = g.vox_base + (((long long)ix * ny + iy) * nz + iz);
-                    const unsigned bit = 1u << (v & 31);
-                    const unsigned old = atomicOr(bitmap + (v >> 5), bit);
-                    if (!(old & bit)) {
-                        const unsigned long long slot = atomicAdd(fix, 1ull);
-                        if (slot < cap) fix[FIX_HDR + slot] = (unsigned long long)v;
-                    }
+            for (int q = 0; q < 2; ++q) {
+                if (q == 0 ? !fa : !fb) continue;
+                const int ix = ip[0] + (int)(q == 0 ? jxa : jxb);
+                if (ix < 0 || ix >= nx) continue;
+                const long long v = g.vox_base + (((long long)ix * ny + iy) * nz + iz);
+                const unsigned bit = 1u << (v & 31);
+                const unsigned old = atomicOr(bitmap + (v >> 5), bit);
+                if (!(old & bit)) {
+                    const unsigned long long slot = atomicAdd(fix, 1ull);
+                    if (slot < cap) fix[FIX_HDR + slot] = (unsigned long long)v;
                 }
             }
         }

@@ -24,6 +24,8 @@
 //       Output: coalesced 32-byte (8-channel) streaming stores, 4 lanes = one 128-byte line.
 // HBM-bound gather-accumulate: no tensor cores (max of a transcendental is not a contraction).
 #include <cub/device/device_scan.cuh>
+#include <thrust/iterator/counting_iterator.h>
+#include <thrust/iterator/transform_iterator.h>
 #include <cuda.h>  // CUtensorMap (types only; the encoder is looked up through the runtime, libcuda is not linked)
 
 #include <cfloat>
@@ -1088,7 +1090,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         GridDev *d_grids;
         float4 *rec_pos;
         uint4 *rec_tag;
-        unsigned *blk_count, *blk_start, *d_bitmap, *d_queue;
+        unsigned *blk_count, *blk_start, *d_bitmap, *d_queue, *segs = nullptr, *seg_n = nullptr;
         uint2 *blk_ent;
         long long *d_ibase;
         unsigned long long *d_fix;
@@ -1097,10 +1099,17 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         const long long n_words = cdiv(voxels, 32);
         const unsigned fix_cap = (unsigned)std::min<long long>(voxels, 1ll << 22);
         const size_t nslots = (size_t)run_blocks + 1;  // + 1: the total after the exclusive scan
+        const long long list_ctas = cdiv(items, L_THREADS);
         if ((rc = scratch_get(h, S_DESC, (size_t)B, &d_grids))) return rc;
         if ((rc = scratch_get(h, S_SORT_PX, ni, &rec_pos))) return rc;
         if ((rc = scratch_get(h, S_SORT_PY, ni, &rec_tag))) return rc;
-        if ((rc = scratch_get(h, S_CELL_COUNT, nslots, &blk_count))) return rc;
+        // per block: entries in the CTAs' table segments (blk_count), then the direct insertions (blk_direct)
+        if ((rc = scratch_get(h, S_CELL_COUNT, 2 * nslots, &blk_count))) return rc;
+        unsigned *const blk_direct = blk_count + nslots;
+        if (list_table && list_ctas > 0) {  // the count pass's table segments, read back by the fill pass
+            if ((rc = scratch_get(h, S_BLK_SEGS, (size_t)list_ctas * (L_SEG_WORDS + 1), &segs))) return rc;
+            seg_n = segs + (size_t)list_ctas * L_SEG_WORDS;
+        }
         if ((rc = scratch_get(h, S_CELL_START, nslots, &blk_start))) return rc;
         if ((rc = scratch_get(h, S_BLK_ENT, (size_t)std::max<long long>(ent_bound, 1), &blk_ent))) return rc;
         if ((rc = scratch_get(h, S_BLOCK_BASE, (size_t)B + 1, &d_ibase))) return rc;
@@ -1110,8 +1119,12 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         // cub temp storage for the scans, sized before anything is enqueued
         unsigned *scan_tmp = nullptr;
         size_t scan_bytes = 0;
+        const auto list_len = thrust::make_transform_iterator(thrust::counting_iterator<int>(0), ListLength{blk_count, blk_direct});
         {
-            MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, blk_count, blk_start, (int)nslots, st));
+            size_t rank_bytes = 0;
+            MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, list_len, blk_start, (int)nslots, st));
+            MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, rank_bytes, blk_count, blk_start, (int)nslots, st));
+            scan_bytes = std::max(scan_bytes, rank_bytes);
             void *tmp = nullptr;
             if ((rc = scratch_get(h, S_SCAN_TMP, scan_bytes, &tmp))) return rc;
             scan_tmp = static_cast<unsigned *>(tmp);
@@ -1133,7 +1146,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
             MKB_CUDA(h, cudaMemcpyAsync(d_ibase, static_cast<char *>(stage) + gbytes, ibytes, cudaMemcpyHostToDevice, st));
             MKB_CUDA(h, cudaEventRecord(*sev, st));
         }
-        MKB_CUDA(h, cudaMemsetAsync(blk_count, 0, sizeof(unsigned) * nslots, st));
+        MKB_CUDA(h, cudaMemsetAsync(blk_count, 0, sizeof(unsigned) * 2 * nslots, st));
         MKB_CUDA(h, cudaMemsetAsync(d_bitmap, 0, sizeof(unsigned) * (size_t)n_words, st));
         MKB_CUDA(h, cudaMemsetAsync(d_queue, 0, sizeof(unsigned) * 64, st));
         MKB_CUDA(h, cudaMemsetAsync(d_fix, 0, sizeof(unsigned long long) * FIX_HDR, st));
@@ -1152,16 +1165,18 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         }
         h->last_kernel = "occ_fill_runs_kernel";
         if (items > 0) {
-            occ_prep_kernel<<<(unsigned)cdiv(items, L_THREADS), L_THREADS, 0, st>>>(coords, sigmas, radii, chanmask, d_grids, B, items, rec_pos, rec_tag, blk_count, list_table);
+            occ_prep_kernel<<<(unsigned)list_ctas, L_THREADS, 0, st>>>(coords, sigmas, radii, chanmask, d_grids, B, items, rec_pos, rec_tag,
+                                                                       blk_count, blk_direct, segs, seg_n, list_table);
             MKB_LAUNCHED(h);
         }
-        MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, blk_count, blk_start, (int)nslots, st));
+        MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, list_len, blk_start, (int)nslots, st));
         h->launches++;
         if (items > 0) {
-            occ_blk_fill_kernel<<<(unsigned)cdiv(items, L_THREADS), L_THREADS, 0, st>>>(d_grids, B, items, rec_pos, rec_tag, blk_count, blk_start, blk_ent, list_table);
+            occ_blk_fill_kernel<<<(unsigned)list_ctas, L_THREADS, 0, st>>>(d_grids, B, items, rec_pos, rec_tag, blk_direct, blk_start, segs, seg_n,
+                                                                           blk_ent, list_table);
             MKB_LAUNCHED(h);
         }
-        if (blk_rank) {  // record index of every non-empty block (blk_count is free again after the list fill)
+        if (blk_rank) {  // record index of every non-empty block (the flags overwrite all of blk_count, unused after the scan)
             occ_blk_flag_kernel<<<(unsigned)cdiv(run_blocks + 1, 256), 256, 0, st>>>(blk_start, run_blocks, blk_count);
             MKB_LAUNCHED(h);
             MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, blk_count, blk_rank, (int)(run_blocks + 1), st));
