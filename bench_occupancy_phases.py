@@ -8,9 +8,9 @@ Reported per workload: the step time, the median over windows of back-to-back st
 (CUDA events, profiler off); and from torch.profiler with CUDA activities, in a pass of its own, the mean device time
 per step of every kernel, memset and copy, grouped into phases:
   upload     descriptor copy
-  memset     blk_count, band bitmap, queue and fix-list header
+  memset     tile counts and block bits, band bitmap, queue and fix-list header
   band       occ_band_kernel (gate-band pre-pass, on a side stream beside the list build for large batches)
-  prep       occ_prep_kernel (records + per-block counts)
+  prep       occ_prep_kernel (records + per-tile counts and block bits)
   scan       cub ExclusiveSum of the counts
   list_fill  occ_blk_fill_kernel (candidate lists)
   fill       occ_fill_runs_kernel

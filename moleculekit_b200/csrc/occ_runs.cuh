@@ -1,12 +1,15 @@
-// occ_runs.cuh -- K1, the default 8-channel occupancy fill (v10): per-block candidate lists + a persistent "mask-run" kernel.
+// occ_runs.cuh -- K1, the default 8-channel occupancy fill (v10): per-tile candidate lists + a persistent "mask-run" kernel.
 // Included by occupancy.cu (after GridDev / occ_value).  Replaces the inner loop of
 // moleculekit/occupancy_utils/occupancy_utils.pyx:46-61.  DESIGN.md section 3 has the derivations; the superseded variants
 // (float-compare gate with predicated FMNMX, scalar FFMA hot loop, row-copy stores, in-register record gathers, jump-table
 // flush, FFMA.SAT gate ...) are in the git history of this file together with their compile-time selectors.
 //
-//   * K2' (occ_prep_kernel / occ_blk_fill_kernel): every atom is appended to the candidate list of each 4x4x8-voxel
-//     block it can reach (~16 blocks per atom at 1 A) -- count (per CTA and block in shared memory, reserving the CTA's
-//     list segments), scan, fill (one walk).  The fill kernel reads its list; no block scans cell rows.
+//   * K2' (occ_prep_kernel / occ_blk_fill_kernel): the reach test is per 4x4x8-voxel block (~16 blocks per atom at 1 A),
+//     the candidate lists are per tile = 2 x 2 x 1 blocks = 8x8x8 voxels (~6 tiles per atom): an atom is appended once to
+//     the list of each tile with a block in reach, and the entry carries one bit per block of the tile -- count (per CTA
+//     and tile in shared memory, reserving the CTA's list segments), scan, fill (one walk).  The fill kernel reads the
+//     list of its block's tile and keeps the entries with the block's bit: the candidates of a block are those of a
+//     per-block list.  No block scans cell rows.
 //   * value = max_a [d2 < cut2] f(sigma^2 / d2) with f monotone: the kernel tracks  r = d2 / sigma^2  as a MIN and applies f
 //     once per voxel-channel; no reciprocal per pair.
 //   * One warp owns a block; a lane owns the 4 voxels of one x-row (they share dy, dz).  The candidate is WARP-UNIFORM (two
@@ -40,6 +43,7 @@ constexpr int R_BZ = 8;          // block = 4 x 4 x 8 voxels
 #define MKB_R_CAP 224
 #endif
 constexpr int R_CAP = MKB_R_CAP;  // candidates per round (the 4 KB output stage aliases the records)
+constexpr int R_BATCH = 128;      // list entries a round loads at a time (8 bytes of registers per lane and 32 entries)
 #ifndef MKB_R_WARPS
 #define MKB_R_WARPS 4
 #endif
@@ -51,8 +55,9 @@ constexpr int R_WARPS = MKB_R_WARPS;
 #define MKB_R_ZC 4               // consecutive z blocks per queue item
 #endif
 constexpr int R_ZC = MKB_R_ZC;
-// per warp and candidate: x differences 16 | (-y, -z, w, tag) 16 | mask 1 | rank 1 bytes, then the 512-byte histogram
-constexpr int R_WARP_BYTES = ((R_CAP * 34 + 512 + 127) / 128) * 128;
+// per warp and candidate: x differences 16 | (-y, -z, w, tag) 16 | mask 1 | mask and rank of the kept list entry 2 bytes, then
+// the 512-byte histogram and 4 bytes per candidate for the kept entry's atom item
+constexpr int R_WARP_BYTES = ((R_CAP * 39 + 512 + 127) / 128) * 128;
 static_assert(R_CAP % 32 == 0 && R_CAP * 32 >= 4096 && R_WARP_BYTES % 128 == 0, "bad R_CAP");
 constexpr float R_GATE_HUGE = 8.507059173023462e37f;  // 2^126: the epilogue's "no atom reached this voxel-channel" bound
 constexpr float R_LIST_SLACK = 2e-4f;                 // relative slack of the block lists' reach test (float32 positions)
@@ -62,8 +67,9 @@ struct RunParams {
     int B;
     const float4 *rec_pos;       // per atom item: position minus its nearest lattice point (voxel units), -
     const uint4 *rec_tag;        // mask | multi << 8 | lattice z << 16, atom row, lattice x | y << 16, 1/sigma
-    const unsigned *blk_start;   // [blocks + 1] exclusive offsets of the per-block candidate lists
-    const uint2 *blk_ent;        // (atom item, mask | multi << 8)
+    const unsigned *blk_start;   // [tile slots + 1] exclusive offsets of the per-tile candidate lists
+    const unsigned *tile_bits;   // per tile slot: bit k = block k of the tile has a candidate
+    const uint2 *blk_ent;        // (atom item, mask | multi << 8 | block bits << 9)
     const double *sigmas;        // multi-sigma atoms only
     float *out;
     const long long *item_base;  // [B + 1]: first queue item of every grid (item = 4 x 4 voxels in x, y and R_ZC blocks in z)
@@ -80,58 +86,81 @@ struct RunParams {
     // uniform batches: descriptor of the first grid + strides (constant-bank operands)
     GridDev u;
     long long u_out_stride;
-    unsigned u_ipg, u_nby, u_nzc, u_bpg;  // items per grid, y blocks, z chunks, blocks per grid
+    unsigned u_ipg, u_nby, u_nzc, u_bpg, u_tpg;  // items per grid, y blocks, z chunks, blocks per grid, tile slots per grid
 };
 
 // ---------------------------------------------------------------------------------------------------------
-// K2': records in atom order + per-block candidate lists.
+// K2': records in atom order + per-tile candidate lists.
 // ---------------------------------------------------------------------------------------------------------
-// blocks (4 x 4 x 8 voxels, voxel centres at integers) within `reach` of the point p; f(block id inside the grid)
+// A tile is 2 x 2 x 1 blocks; block (bx, by, bz) is bit block_bit(bx, by) of tile (bx >> 1, by >> 1, bz), whose list slot
+// inside the grid is tile_slot().  Consecutive z blocks are consecutive slots.  A grid with an odd number of blocks in x or
+// y has tiles with missing blocks; their bits are never set.
+__host__ __device__ __forceinline__ long long tile_slot(int nty, int nbz, int bx, int by, int bz) {
+    return ((long long)(bx >> 1) * nty + (by >> 1)) * nbz + bz;
+}
+__host__ __device__ __forceinline__ unsigned block_bit(int bx, int by) { return (unsigned)((bx & 1) * 2 + (by & 1)); }
+constexpr int L_ENT_BITS = 9;  // a list entry's block bits sit above mask | multi << 8
+
+// tiles with a block (4 x 4 x 8 voxels, voxel centres at integers) within `reach` of the point p; f(tile slot inside the
+// grid, bits of the blocks in reach)
 template <class F>
-__device__ __forceinline__ void for_each_block_in_reach(const GridDev &g, float px, float py, float pz, F f) {
+__device__ __forceinline__ void for_each_tile_in_reach(const GridDev &g, float px, float py, float pz, F f) {
     const int nbx = (g.dims[0] + 3) >> 2, nby = (g.dims[1] + 3) >> 2, nbz = (g.dims[2] + R_BZ - 1) / R_BZ;
+    const int nty = (nby + 1) >> 1;
     const float reach2 = g.cut2v * (1.0f + R_LIST_SLACK);
     const float reach = sqrtf(reach2) * (1.0f + 1e-6f);
     const int bx0 = max(0, (int)ceilf((px - reach - 3.0f) * 0.25f)), bx1 = min(nbx - 1, (int)floorf((px + reach) * 0.25f));
     const int by0 = max(0, (int)ceilf((py - reach - 3.0f) * 0.25f)), by1 = min(nby - 1, (int)floorf((py + reach) * 0.25f));
     const int bz0 = max(0, (int)ceilf((pz - reach - 7.0f) * 0.125f)), bz1 = min(nbz - 1, (int)floorf((pz + reach) * 0.125f));
-    for (int bx = bx0; bx <= bx1; ++bx) {
-        const float dx = fmaxf(fmaxf((float)(4 * bx) - px, px - (float)(4 * bx + 3)), 0.0f);
-        for (int by = by0; by <= by1; ++by) {
-            const float dy = fmaxf(fmaxf((float)(4 * by) - py, py - (float)(4 * by + 3)), 0.0f);
-            const float dxy = fmaf(dy, dy, dx * dx);
-            if (dxy > reach2) continue;
+    const float INF = __int_as_float(0x7f800000);
+    for (int tx = bx0 >> 1; tx <= bx1 >> 1; ++tx) {
+        for (int ty = by0 >> 1; ty <= by1 >> 1; ++ty) {
+            // squared x-y distance to the tile's four blocks; +inf for a block outside the atom's block range (or the grid)
+            float dxy[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const int bx = 2 * tx + (q >> 1), by = 2 * ty + (q & 1);
+                const float dx = fmaxf(fmaxf((float)(4 * bx) - px, px - (float)(4 * bx + 3)), 0.0f);
+                const float dy = fmaxf(fmaxf((float)(4 * by) - py, py - (float)(4 * by + 3)), 0.0f);
+                dxy[q] = (bx >= bx0 && bx <= bx1 && by >= by0 && by <= by1) ? fmaf(dy, dy, dx * dx) : INF;
+            }
+            if (fminf(fminf(dxy[0], dxy[1]), fminf(dxy[2], dxy[3])) > reach2) continue;
             for (int bz = bz0; bz <= bz1; ++bz) {
                 const float dz = fmaxf(fmaxf((float)(R_BZ * bz) - pz, pz - (float)(R_BZ * bz + R_BZ - 1)), 0.0f);
-                if (fmaf(dz, dz, dxy) <= reach2) f((bx * nby + by) * nbz + bz);
+                unsigned bits = 0;
+#pragma unroll
+                for (int q = 0; q < 4; ++q) bits |= (fmaf(dz, dz, dxy[q]) <= reach2 ? 1u : 0u) << q;
+                if (bits) f((int)tile_slot(nty, nbz, 2 * tx, 2 * ty, bz), bits);
             }
         }
     }
 }
 
-// The atoms of one CTA share most of their blocks (C3: ~4 200 insertions into ~700 blocks per 256 atoms), so the count
-// pass counts per (CTA, block) in a shared-memory hash table keyed by the global block slot (tile_base + block id; a CTA
-// may span several grids; linear probing) and touches global memory once per occupied entry.  An insertion whose key
-// finds neither itself nor a free slot within L_PROBES slots is counted in global memory directly (blk_direct).  Keys
-// are never removed, so within a CTA a key is either entirely in the table or entirely direct, and a table rebuilt with
-// every key at its slot routes each insertion as the count pass did.  At fine voxel sizes the atoms of a CTA reach far
-// more blocks than the table holds (C5, 0.5 A: ~100 blocks per atom, ~9 000 per CTA); there the host turns the table off
-// (`table` = 0) and every insertion takes the direct route.
+// The atoms of one CTA share most of their tiles, so the count pass counts per (CTA, tile) in a shared-memory hash table
+// keyed by the global tile slot (tile_base + slot inside the grid; a CTA may span several grids; linear probing) and
+// touches global memory once per occupied entry: the count, and the OR of the insertions' block bits (tile_bits).  An
+// insertion whose key finds neither itself nor a free slot within L_PROBES slots is counted in global memory directly
+// (blk_direct).  Keys are never removed, so within a CTA a key is either entirely in the table or entirely direct, and a
+// table rebuilt with every key at its slot routes each insertion as the count pass did.  Where an atom can reach more
+// than L_TABLE_MAX_REACH tiles the atoms of a CTA reach more tiles than the table holds; there the host turns the table
+// off (`table` = 0) and every insertion takes the direct route.
 //
-// The list of block k spans [blk_start[k], blk_start[k + 1]) = blk_count[k] in-table entries + blk_direct[k] direct ones.
+// The list of tile k spans [blk_start[k], blk_start[k + 1]) = blk_count[k] in-table entries + blk_direct[k] direct ones.
 // The direct entries fill it from the front, the in-table segments from the back: the count pass's
 // atomicAdd(blk_count + k, n) returns the CTA's segment base b, and the segment is [blk_start[k + 1] - b - n, .. - b).
 constexpr int L_THREADS = 256;          // atoms per CTA of the two list passes
 constexpr int L_TABLE = 2048;           // hash slots per CTA (power of two)
 constexpr int L_PROBES = 8;             // linear-probing limit
 constexpr int L_STAGE = 4096;           // entries per CTA staged in shared memory by the fill pass
-constexpr int L_TABLE_MAX_REACH = 64;   // the host uses the table when an atom reaches at most this many blocks
+constexpr int L_TABLE_MAX_REACH = 64;   // the host uses the table when an atom reaches at most this many tiles
 constexpr unsigned L_EMPTY = 0xffffffffu;
 constexpr int L_SLOTS = L_TABLE / L_THREADS;  // slots per thread in the fill pass's scan
 constexpr int L_SEG_WORDS = 3 * L_TABLE;      // per CTA: the keys, segment bases and slot | n << 11 of its occupied slots
-static_assert(L_TABLE <= 2048 && L_THREADS <= 256, "a staged entry packs slot (11 bits) | thread (8) | mask (9)");
+constexpr int L_CNT_BITS = 28;          // a table counter: insertions | block bits << L_CNT_BITS
+static_assert(L_TABLE <= 2048 && L_THREADS <= 256 && L_ENT_BITS + 4 == 13,
+              "a staged entry packs slot (11 bits) | thread (8) | mask, multi and block bits (13)");
 
-// scan input: the length of block i's list
+// scan input: the length of tile slot i's list
 struct ListLength {
     const unsigned *count, *direct;
     __host__ __device__ unsigned operator()(int i) const { return count[i] + direct[i]; }
@@ -164,13 +193,13 @@ __device__ __forceinline__ void list_table_clear(unsigned *s_key, unsigned *s_cn
     for (int i = threadIdx.x; i < L_TABLE; i += L_THREADS) { s_key[i] = L_EMPTY; s_cnt[i] = 0u; }
 }
 
-// per atom item: record + block counts.  sigma handling as occ_scatter_kernel (one sigma + channel mask; several
+// per atom item: record + tile counts and block bits.  sigma handling as occ_scatter_kernel (one sigma + channel mask; several
 // distinct sigmas -> multi flag and the per-channel path of the fill kernel).
 __device__ __forceinline__ void occ_prep_item(const float *__restrict__ coords, const double *__restrict__ sigmas,
                                               const double *__restrict__ radii, const unsigned *__restrict__ chanmask,
                                               const GridDev *__restrict__ grids, int B, long long it, float4 *__restrict__ rec_pos,
-                                              uint4 *__restrict__ rec_tag, unsigned *__restrict__ blk_direct, int table,
-                                              unsigned *s_key, unsigned *s_cnt) {
+                                              uint4 *__restrict__ rec_tag, unsigned *__restrict__ blk_direct,
+                                              unsigned *__restrict__ tile_bits, int table, unsigned *s_key, unsigned *s_cnt) {
     const int b = find_grid_item(grids, B, it);
     const GridDev &g = grids[b];
     const long long a = g.atom_begin + (it - g.item_base);
@@ -211,15 +240,20 @@ __device__ __forceinline__ void occ_prep_item(const float *__restrict__ coords, 
     rec_tag[it] = make_uint4(live ? (m | (multi ? 0x100u : 0u) | ((unsigned)(ip[2] + off) << 16)) : 0u, (unsigned)a,
                              live ? ((unsigned)(ip[0] + off) | ((unsigned)(ip[1] + off) << 16)) : 0u, __float_as_uint(sw));
     if (!live) return;
-    const unsigned tb = (unsigned)g.tile_base;  // first block slot of this grid
-    for_each_block_in_reach(g, (float)ip[0] + f[0], (float)ip[1] + f[1], (float)ip[2] + f[2], [&](int bid) {
-        const int s = table ? list_slot_insert(s_key, tb + bid) : -1;
-        if (s >= 0) atomicAdd(s_cnt + s, 1u);
-        else atomicAdd(blk_direct + tb + bid, 1u);
+    const unsigned tb = (unsigned)g.tile_base;  // first tile slot of this grid
+    for_each_tile_in_reach(g, (float)ip[0] + f[0], (float)ip[1] + f[1], (float)ip[2] + f[2], [&](int tid, unsigned bits) {
+        const int s = table ? list_slot_insert(s_key, tb + tid) : -1;
+        if (s >= 0) {
+            const unsigned old = atomicAdd(s_cnt + s, 1u);  // the bits saturate after a few insertions: mostly one atomic
+            if (bits & ~(old >> L_CNT_BITS)) atomicOr(s_cnt + s, bits << L_CNT_BITS);
+        } else {
+            atomicAdd(blk_direct + tb + tid, 1u);
+            atomicOr(tile_bits + tb + tid, bits);
+        }
     });
 }
 
-// count pass: records, then per occupied table slot one atomicAdd reserves the CTA's segment of that block's list; with
+// count pass: records, then per occupied table slot one atomicAdd reserves the CTA's segment of that tile's list; with
 // the table on, the CTA keeps (key, base, slot | n << 11) of every occupied slot, compacted, in its L_SEG_WORDS of `segs`
 // and their number in seg_n[CTA] for the fill pass.
 __global__ void __launch_bounds__(L_THREADS) occ_prep_kernel(const float *__restrict__ coords, const double *__restrict__ sigmas,
@@ -227,13 +261,14 @@ __global__ void __launch_bounds__(L_THREADS) occ_prep_kernel(const float *__rest
                                                              const GridDev *__restrict__ grids, int B, long long n_items,
                                                              float4 *__restrict__ rec_pos, uint4 *__restrict__ rec_tag,
                                                              unsigned *__restrict__ blk_count, unsigned *__restrict__ blk_direct,
-                                                             unsigned *__restrict__ segs, unsigned *__restrict__ seg_n, int table) {
+                                                             unsigned *__restrict__ tile_bits, unsigned *__restrict__ segs,
+                                                             unsigned *__restrict__ seg_n, int table) {
     __shared__ unsigned s_key[L_TABLE], s_cnt[L_TABLE], s_nseg;
     list_table_clear(s_key, s_cnt);
     if (threadIdx.x == 0) s_nseg = 0u;
     __syncthreads();
     const long long it = blockIdx.x * (long long)L_THREADS + threadIdx.x;
-    if (it < n_items) occ_prep_item(coords, sigmas, radii, chanmask, grids, B, it, rec_pos, rec_tag, blk_direct, table, s_key, s_cnt);
+    if (it < n_items) occ_prep_item(coords, sigmas, radii, chanmask, grids, B, it, rec_pos, rec_tag, blk_direct, tile_bits, table, s_key, s_cnt);
     if (!table) return;
     __syncthreads();
     unsigned *const seg = segs + (size_t)blockIdx.x * L_SEG_WORDS;
@@ -246,9 +281,10 @@ __global__ void __launch_bounds__(L_THREADS) occ_prep_kernel(const float *__rest
         if (lane == 0 && occ) j0 = atomicAdd(&s_nseg, (unsigned)__popc(occ));
         j0 = __shfl_sync(0xffffffffu, j0, 0);
         if (key != L_EMPTY) {
-            const unsigned n = s_cnt[i], j = j0 + __popc(occ & ((1u << lane) - 1u));
+            const unsigned c = s_cnt[i], n = c & ((1u << L_CNT_BITS) - 1u), j = j0 + __popc(occ & ((1u << lane) - 1u));
             seg[j] = key;
             seg[L_TABLE + j] = atomicAdd(blk_count + key, n);
+            atomicOr(tile_bits + key, c >> L_CNT_BITS);
             seg[2 * L_TABLE + j] = (unsigned)i | n << 11;
         }
     }
@@ -256,10 +292,10 @@ __global__ void __launch_bounds__(L_THREADS) occ_prep_kernel(const float *__rest
     if (threadIdx.x == 0) seg_n[blockIdx.x] = s_nseg;
 }
 
-// fill pass: the same walk appends (item, mask | multi << 8) to the lists.  The CTA puts the count pass's occupied slots
+// fill pass: the same walk appends (item, mask | multi << 8 | block bits << 9) to the lists.  The CTA puts the count pass's occupied slots
 // back at their slot indices (the same slots, so list_slot_find routes every insertion as the count pass did) and one walk
 // places each in-table insertion at its segment's start + a shared cursor.  The first L_STAGE entries of the CTA are
-// staged in shared memory in segment order (one word: table slot, thread, mask) and leave in one pass at the end,
+// staged in shared memory in segment order (one word: table slot, thread, mask and bits) and leave in one pass at the end,
 // consecutive threads writing consecutive list positions (one scattered 8-byte store per entry took most of the pass);
 // entries beyond L_STAGE are stored at once.  Direct insertions take their position one by one from blk_direct, which
 // counts down to zero.
@@ -331,15 +367,15 @@ __global__ void __launch_bounds__(L_THREADS, 5) occ_blk_fill_kernel(const GridDe
     if (live) {
         const unsigned tb = (unsigned)g->tile_base;
         const uint2 ent = make_uint2((unsigned)it, tg.x & 0x1ffu);
-        for_each_block_in_reach(*g, px, py, pz, [&](int bid) {
-            const unsigned key = tb + bid;
+        for_each_tile_in_reach(*g, px, py, pz, [&](int tid, unsigned bits) {
+            const unsigned key = tb + tid, ey = ent.y | bits << L_ENT_BITS;
             const int s = list_slot_find(s_key, key);
             if (s >= 0) {
                 const unsigned li = atomicAdd(s_cur + s, 1u);
-                if (li < (unsigned)L_STAGE) s_stage[li] = (unsigned)s << 17 | threadIdx.x << 9 | ent.y;
-                else blk_ent[s_off[s] + li] = ent;
+                if (li < (unsigned)L_STAGE) s_stage[li] = (unsigned)s << 21 | threadIdx.x << 13 | ey;
+                else blk_ent[s_off[s] + li] = make_uint2(ent.x, ey);
             } else {
-                blk_ent[blk_start[key] + atomicSub(blk_direct + key, 1u) - 1u] = ent;
+                blk_ent[blk_start[key] + atomicSub(blk_direct + key, 1u) - 1u] = make_uint2(ent.x, ey);
             }
         });
     }
@@ -347,14 +383,29 @@ __global__ void __launch_bounds__(L_THREADS, 5) occ_blk_fill_kernel(const GridDe
     const unsigned it0 = (unsigned)(blockIdx.x * L_THREADS);
     for (unsigned i = threadIdx.x; i < min(total, (unsigned)L_STAGE); i += L_THREADS) {
         const unsigned w = s_stage[i];
-        blk_ent[s_off[w >> 17] + i] = make_uint2(it0 + ((w >> 9) & 0xffu), w & 0x1ffu);
+        blk_ent[s_off[w >> 21] + i] = make_uint2(it0 + ((w >> 13) & 0xffu), w & 0x1fffu);
     }
 }
 
-// compact output: 1 for every block with a candidate list, then an exclusive scan gives its record index
-__global__ void occ_blk_flag_kernel(const unsigned *__restrict__ blk_start, long long n_blocks, unsigned *__restrict__ flag) {
+// compact output: 1 for every block with a candidate (its bit of its tile), then an exclusive scan gives its record index
+__global__ void occ_blk_flag_kernel(const GridDev *__restrict__ grids, int B, const unsigned *__restrict__ tile_bits,
+                                    long long n_blocks, unsigned *__restrict__ flag) {
     const long long b = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    if (b <= n_blocks) flag[b] = (b < n_blocks && blk_start[b + 1] != blk_start[b]) ? 1u : 0u;
+    if (b > n_blocks) return;
+    unsigned f = 0u;
+    if (b < n_blocks) {
+        int lo = 0, hi = B - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (grids[mid].blk_base <= b) lo = mid; else hi = mid - 1;
+        }
+        const GridDev &g = grids[lo];
+        const int nby = (g.dims[1] + 3) >> 2, nbz = (g.dims[2] + R_BZ - 1) / R_BZ;
+        const long long bxy = (b - g.blk_base) / nbz;
+        const int bz = (int)((b - g.blk_base) % nbz), by = (int)(bxy % nby), bx = (int)(bxy / nby);
+        f = (tile_bits[g.tile_base + tile_slot((nby + 1) >> 1, nbz, bx, by, bz)] >> block_bit(bx, by)) & 1u;
+    }
+    flag[b] = f;
 }
 
 __device__ __forceinline__ void bulk_store_row(float *dst, unsigned src_smem, int bytes) {
@@ -402,8 +453,9 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
     float4 *const rec = reinterpret_cast<float4 *>(wb);                         // sorted candidates: the four x differences, x lambda
     float4 *const recy = reinterpret_cast<float4 *>(wb + R_CAP * 16);           // (-y lambda, -z lambda, w, tag: mask | flags)
     unsigned char *const msk = wb + R_CAP * 32;                                 // channel mask of the sorted candidate
-    unsigned char *const rnk = wb + R_CAP * 33;                                 // rank of a candidate inside its mask bin
-    unsigned *const hist = reinterpret_cast<unsigned *>(wb + R_CAP * 34);       // 256 x 16-bit bins in 128 words
+    unsigned short *const crm = reinterpret_cast<unsigned short *>(wb + R_CAP * 33);  // kept entry: mask | rank inside its mask bin << 8
+    unsigned *const hist = reinterpret_cast<unsigned *>(wb + R_CAP * 35);       // 256 x 16-bit bins in 128 words
+    unsigned *const cix = reinterpret_cast<unsigned *>(wb + R_CAP * 35 + 512);  // kept entry: atom item
     // the hot loop loads through an address the compiler cannot rematerialise (it would rebuild it from S2R SR_TID /
     // SR_CgaCtaId at the head of every run: ten instructions and two slow special-register reads)
     unsigned rec_sa = (unsigned)__cvta_generic_to_shared(wb);
@@ -470,10 +522,15 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
         const float cut2 = RG(cut2v);
         const int off = RG(cutv) + 1;
         const int bz_begin = zc * p.zc, bz_end = min(nbz, bz_begin + p.zc);
-        // candidate list offsets of the item's blocks (consecutive block ids): lanes 0..R_ZC
-        const long long blk0 = (UNIFORM ? p.u.tile_base + (long long)gi * p.u_bpg : __ldg(&gg->tile_base)) + (long long)bxy * nbz + bz_begin;
-        const unsigned my_start = __ldg(p.blk_start + blk0 + min(lane, bz_end - bz_begin));
-        if (__shfl_sync(0xffffffffu, my_start, bz_end - bz_begin) == __shfl_sync(0xffffffffu, my_start, 0)) {
+        // candidate list offsets of the tiles of the item's blocks (consecutive tile slots): lanes 0..R_ZC; beside them the
+        // tiles' block bits: `has` bit k = an atom reaches the item's block k
+        const long long tile0 = (UNIFORM ? p.u.tile_base + (long long)gi * p.u_tpg : __ldg(&gg->tile_base)) +
+                                tile_slot((int)(nby + 1) >> 1, nbz, bxi, byi, bz_begin);
+        const unsigned keep = (1u << L_ENT_BITS) << block_bit(bxi, byi);  // this block's bit in a list entry
+        const unsigned my_start = __ldg(p.blk_start + tile0 + min(lane, bz_end - bz_begin));
+        const unsigned my_bits = __ldg(p.tile_bits + tile0 + min(lane, bz_end - bz_begin - 1));
+        const unsigned has = __ballot_sync(0xffffffffu, lane < bz_end - bz_begin && ((my_bits << L_ENT_BITS) & keep));
+        if (has == 0u) {
             // no atom reaches any block of the item: one bulk copy of zeros per output row (TMA, nothing to wait for)
             const int z0 = bz_begin * R_BZ;
             if (p.blk_rank) {
@@ -500,9 +557,7 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
             const int z0 = bzi * R_BZ;
             const int row_bytes = min(R_BZ, nz - z0) * 32;
             float *const row_dst = row_base + z0 * 8;
-            const unsigned ls = __shfl_sync(0xffffffffu, my_start, bzi - bz_begin);
-            const unsigned n = __shfl_sync(0xffffffffu, my_start, bzi - bz_begin + 1) - ls;
-            if (n == 0) {
+            if (!((has >> (bzi - bz_begin)) & 1u)) {
                 if (p.blk_rank) {
                 } else if (p.cmajor) {
                     store_cmajor_zero(p.out + out_offset * 8, nx, ny, nz, x0, y0 + ly, z0 + lz);
@@ -518,6 +573,9 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
                 continue;
             }
 
+            // the tile's list: the entries without this block's bit belong to the tile's other blocks
+            const unsigned ls = __shfl_sync(0xffffffffu, my_start, bzi - bz_begin);
+            const unsigned n = __shfl_sync(0xffffffffu, my_start, bzi - bz_begin + 1) - ls;
             float acc[8][4];
 #pragma unroll
             for (int h = 0; h < 8; ++h)
@@ -526,41 +584,51 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
             // lattice point of the block corner in the records' offset frame
             const int cx = x0 + off, cy = y0 + off, cz = z0 + off;
 
-            for (unsigned base = 0; base < n; base += R_CAP) {
-                const int np = (int)min((unsigned)R_CAP, n - base);
+            for (unsigned base = 0, span; base < n; base += span) {
                 const uint2 *const ent = p.blk_ent + ls + base;
-                // ---- pass 1: histogram of the channel masks, rank of every candidate inside its bin
-                unsigned ey[R_CAP / 32];
-                {
-#pragma unroll
-                    for (int u = 0; u < R_CAP / 32; ++u) {  // all loads of the round in flight together
-                        const int j = u * 32 + lane;
-                        ey[u] = j < np ? __ldg(&ent[j].y) : 0u;
-                    }
-                }
+                // ---- pass 1: the tile's list entries that carry this block's bit are the block's candidates; they are
+                // compacted (atom item, mask, rank inside the mask's bin) next to the histogram of the channel masks.  A
+                // round takes list entries, R_BATCH at a time with all loads in flight, until it holds more than R_CAP - 32
+                // candidates or the list ends: `span` entries, nk candidates
+                int nk = 0;
+                span = 0;
                 // the histogram trips carry no other code: the per-channel path of multi-sigma atoms (rare: user float channels) used
                 // to be inlined in each of the R_CAP / 32 unrolled trips -- 34 KB of code that the instruction cache had to skip
                 bool any_multi = false;
+                do {
+                    const int np = (int)min((unsigned)R_BATCH, n - base - span);
+                    uint2 e[R_BATCH / 32];
 #pragma unroll
-                for (int u = 0; u < R_CAP / 32; ++u) {
-                    const int j0 = u * 32;
-                    if (j0 >= np) break;
-                    const int j = j0 + lane;
-                    const uint2 e = make_uint2(0u, ey[u]);
-                    const bool multi = (e.y & 0x100u) != 0;
-                    any_multi |= multi;
-                    if (j < np) {
-                        const unsigned m = multi ? 0u : (e.y & 255u), sh = (m & 1u) * 16u;
-                        const unsigned old = atomicAdd(&hist[m >> 1], 1u << sh);
-                        rnk[j] = (unsigned char)((old >> sh) & 0xffffu);
+                    for (int u = 0; u < R_BATCH / 32; ++u) {
+                        const int j = u * 32 + lane;
+                        e[u] = j < np ? __ldg(ent + span + j) : make_uint2(0u, 0u);
                     }
-                }
+                    const unsigned span0 = span;
+#pragma unroll
+                    for (int u = 0; u < R_BATCH / 32; ++u) {
+                        if (u * 32 >= np || nk > R_CAP - 32) break;
+                        const bool kept = (e[u].y & keep) != 0;  // false past the end of the list
+                        const unsigned kb = __ballot_sync(0xffffffffu, kept);
+                        const bool multi = kept && (e[u].y & 0x100u) != 0;
+                        any_multi |= multi;
+                        if (kept) {
+                            const unsigned m = multi ? 0u : (e[u].y & 255u), sh = (m & 1u) * 16u;
+                            const unsigned old = atomicAdd(&hist[m >> 1], 1u << sh);
+                            const int k = nk + __popc(kb & ((1u << lane) - 1u));
+                            cix[k] = e[u].x;
+                            crm[k] = (unsigned short)(m | ((old >> sh) & 0xffu) << 8);
+                        }
+                        nk += __popc(kb);
+                        span = span0 + min(u * 32 + 32, np);
+                    }
+                } while (base + span < n && nk <= R_CAP - 32);
+                const int np = (int)span;
                 if (__any_sync(0xffffffffu, any_multi)) {
 #pragma unroll 1
                     for (int j0 = 0; j0 < np; j0 += 32) {
                         const int j = j0 + lane;
                         const uint2 e = j < np ? __ldg(ent + j) : make_uint2(0u, 0u);
-                        const bool multi = (e.y & 0x100u) != 0;
+                        const bool multi = (e.y & keep) && (e.y & 0x100u);
                     // atoms with several distinct sigmas (user float channels): whole-warp per-channel path; they stay in
                         // the list under mask 0 (a run that updates no channel)
                         for (unsigned bm = __ballot_sync(0xffffffffu, multi); bm; bm &= bm - 1) {
@@ -622,18 +690,17 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
                 // ---- pass 2: records in run order, scaled by lambda (float64 rebase: one rounding per coordinate); the tag of the
                 // record that closes a run carries the run's mask and the flags of the run loop.
                 // sub-pass a: the raw per-atom data of every candidate goes straight to its sorted slot (cp.async, all in flight)
-                for (int j = lane; j < np; j += 32) {
-                    const uint2 e = __ldg(ent + j);
-                    const unsigned m = (e.y & 0x100u) ? 0u : (e.y & 255u);
-                    const unsigned pos = ((hist[m >> 1] >> ((m & 1u) * 16u)) & 0xffffu) - 1u - (unsigned)rnk[j];
-                    cp_async16(rec_sa + 16u * pos, p.rec_pos + e.x);
-                    cp_async16(rec_sa + (unsigned)(R_CAP * 16) + 16u * pos, p.rec_tag + e.x);
+                for (int j = lane; j < nk; j += 32) {
+                    const unsigned it = cix[j], m = crm[j] & 255u;
+                    const unsigned pos = ((hist[m >> 1] >> ((m & 1u) * 16u)) & 0xffffu) - 1u - (unsigned)(crm[j] >> 8);
+                    cp_async16(rec_sa + 16u * pos, p.rec_pos + it);
+                    cp_async16(rec_sa + (unsigned)(R_CAP * 16) + 16u * pos, p.rec_tag + it);
                     msk[pos] = (unsigned char)m;
                 }
                 asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
                 __syncwarp();
                 // sub-pass b: slot by slot in place (a lane reads and writes its own slots only)
-                for (int j = lane; j < np; j += 32) {
+                for (int j = lane; j < nk; j += 32) {
                     const unsigned pos = (unsigned)j;
                     const unsigned m = msk[pos];
                     const unsigned rk = (((hist[m >> 1] >> ((m & 1u) * 16u)) & 0xffffu) - 1u == pos) ? 0u : 1u;  // 0: closes its run
@@ -653,15 +720,17 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
                     const unsigned e0 = (hist[m >> 1] >> ((m & 1u) * 16u)) & 0xffffu, e1 = (hist[mh >> 1] >> 16) & 0xffffu;
                     recy[pos] = make_float4(-(float)(ey * lam), -(float)(ez * lam), wt,
                                             __uint_as_float(m | ((rk == 0 && e0 == e1) ? 0x100u : 0u) | (rk == 0 ? 0x80000000u : 0u) |
-                                                            (pos + 1u == (unsigned)np ? 0x200u : 0u)));
+                                                            (pos + 1u == (unsigned)nk ? 0x200u : 0u)));
                 }
                 __syncwarp();
                 *reinterpret_cast<uint4 *>(hist + 4 * lane) = make_uint4(0u, 0u, 0u, 0u);
                 __syncwarp();
 
                 // ---- the hot loop: one warp-uniform candidate per half trip, 4 voxels per lane; two records in flight
-                // (a / b ping-pong, the next one is loaded before the current one is evaluated)
-                {
+                // (a / b ping-pong, the next one is loaded before the current one is evaluated).  It reads record 0
+                // unconditionally; a round ends at the end of the list or full, so it holds a candidate whenever tile_bits
+                // has this block's bit
+                if (nk > 0) {
 #define MKB_LDREC(I) lds_rec4(rec_sa + 16u * (unsigned)(I))
 #define MKB_LDRECY(I) lds_rec4(rec_sa + (unsigned)(R_CAP * 16) + 16u * (unsigned)(I))
 #define MKB_RUN_R2(D, Y, R)                                                                       \
@@ -675,7 +744,7 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
         R##3 = __fmul_rn(fmaf(D.w, D.w, s2_), Y.z);                                               \
     }
                     float4 a = MKB_LDREC(0), ya = MKB_LDRECY(0);
-                    int i = 1;  // next record to load; i == np reads past the list (inside this warp's buffer), never used
+                    int i = 1;  // next record to load; i == nk reads past the list (inside this warp's buffer), never used
                     float M0 = INF, M1 = INF, M2 = INF, M3 = INF;
                     // one trip per run; bit 9 of the tag marks the last record of the round (ptxas otherwise rebuilds the candidate
                     // count for a compare at the end of every run)
@@ -781,7 +850,9 @@ __global__ void __launch_bounds__(R_WARPS * 32, MKB_R_MIN_CTAS) occ_fill_runs_ke
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             __syncwarp();
             if (p.blk_rank && !p.sparse_dense) {  // compact output: the whole 4 KB stage is one record, one bulk copy
-                if (lane == 0) bulk_store_row(p.out + 1024ll * __ldg(p.blk_rank + blk0 + (bzi - bz_begin)), stage_sa, 4096);
+                const long long blk = (UNIFORM ? p.u.blk_base + (long long)gi * p.u_bpg : __ldg(&gg->blk_base)) +
+                                      ((long long)(x0 >> 2) * nby + (y0 >> 2)) * nbz + bzi;
+                if (lane == 0) bulk_store_row(p.out + 1024ll * __ldg(p.blk_rank + blk), stage_sa, 4096);
             } else if (p.use_tmap) {
                 if (lane == 0) tma_store_block(&tmap, stage_sa, z0 * 8, y0, x0, gi);
             } else if (row_ok) bulk_store_row(row_dst, stage_sa + lane * 256, row_bytes);
@@ -897,7 +968,7 @@ __global__ void __launch_bounds__(128) occ_band_kernel(const float *__restrict__
 
 // float64 re-evaluation of one voxel with the reference's operations (pyx:46-61): d2 as the reference computes it
 // (centres fl(fl(i*vs) + origin), voxeldescriptors.py:125-132,245), max of sigma^2/d2 per channel, 1 - exp(-q^6).
-// One warp per flagged voxel; the atoms are those of the voxel's block list.
+// One warp per flagged voxel; the atoms are the entries of the voxel's tile list that carry its block's bit.
 __device__ __forceinline__ void occ_fix_voxel(const GridDev *__restrict__ grids, int B, long long v, int lane,
                                               const float *__restrict__ coords, const double *__restrict__ sigmas,
                                               const double *__restrict__ radii, const unsigned *__restrict__ chanmask,
@@ -914,8 +985,11 @@ __device__ __forceinline__ void occ_fix_voxel(const GridDev *__restrict__ grids,
     const int nz = g->dims[2], ny = g->dims[1];
     const int iz = (int)(lv % nz), iy = (int)((lv / nz) % ny), ix = (int)(lv / ((long long)nz * ny));
     const int nby = (ny + 3) >> 2, nbz = (nz + R_BZ - 1) / R_BZ;
-    const long long bid = g->tile_base + ((long long)(ix >> 2) * nby + (iy >> 2)) * nbz + iz / R_BZ;
-    const unsigned e0 = __ldg(blk_start + bid), e1 = __ldg(blk_start + bid + 1);
+    const int bx = ix >> 2, by = iy >> 2, bz = iz / R_BZ;
+    const long long bid = g->blk_base + ((long long)bx * nby + by) * nbz + bz;
+    const long long tid = g->tile_base + tile_slot((nby + 1) >> 1, nbz, bx, by, bz);
+    const unsigned keep = (1u << L_ENT_BITS) << block_bit(bx, by);
+    const unsigned e0 = __ldg(blk_start + tid), e1 = __ldg(blk_start + tid + 1);
     const double cx = __dadd_rn(__dmul_rn((double)ix, g->vs), g->origin[0]);
     const double cy = __dadd_rn(__dmul_rn((double)iy, g->vs), g->origin[1]);
     const double cz = __dadd_rn(__dmul_rn((double)iz, g->vs), g->origin[2]);
@@ -923,7 +997,9 @@ __device__ __forceinline__ void occ_fix_voxel(const GridDev *__restrict__ grids,
 #pragma unroll
     for (int h = 0; h < 8; ++h) q[h] = 0.0;
     for (unsigned i = e0 + lane; i < e1; i += 32) {
-        const unsigned a = __ldg(&rec_tag[__ldg(&blk_ent[i].x)].y);
+        const uint2 e = __ldg(blk_ent + i);
+        if (!(e.y & keep)) continue;
+        const unsigned a = __ldg(&rec_tag[e.x].y);
         const double dx = (double)coords[3ll * a + 0] - cx;
         const double dy = (double)coords[3ll * a + 1] - cy;
         const double dz = (double)coords[3ll * a + 2] - cz;

@@ -61,6 +61,7 @@ struct GridDev {
     long long atom_begin, atom_end, out_offset;
     long long item_base, tile_base, cell_base;
     long long vox_base;  // first voxel of this grid in the dense batch order (gate-band bitmap of the run kernel)
+    long long blk_base;  // run kernel: first 4x4x8 block of this grid (compact records); its lists are per 8x8x8 tile (tile_base)
 };
 
 __device__ __forceinline__ float rcp_approx(float x) {
@@ -1030,6 +1031,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         g.tile_base = tiles;
         g.cell_base = cells;
         g.vox_base = voxels;
+        g.blk_base = 0;
         voxels += (long long)s.dims[0] * s.dims[1] * s.dims[2];
         items += s.atom_end - s.atom_begin;
         tiles += nt;
@@ -1039,7 +1041,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
     if (cells >= (1ll << 31) - 2 || items >= (1ll << 31))
         return fail(h, MKB_ERR_BAD_ARG, "batch too large (%lld cells, %lld atom items): split it", cells, items);
 
-    // ---- default for 8 channels: per-block candidate lists + persistent mask-run kernel with TMA stores (occ_runs.cuh)
+    // ---- default for 8 channels: per-tile candidate lists + persistent mask-run kernel with TMA stores (occ_runs.cuh)
     bool use_runs = fill.runs;
     std::vector<long long> ibase;
     long long run_blocks = 0, run_items = 0, ent_bound = 0;
@@ -1062,9 +1064,11 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
             if (g.dims[0] + 2 * g.cutv + 2 >= 65536 || g.dims[1] + 2 * g.cutv + 2 >= 65536 || g.dims[2] + 2 * g.cutv + 2 >= 65536) use_runs = false;
             nblk[b] = nbx * nby * nbz;
             nitem[b] = nbx * nby * ((nbz + run_zc - 1) / run_zc);
-            // blocks one atom can reach: an interval of 2 cut voxels touches at most floor((2 cut + e - 1) / e) + 1 blocks of edge e
-            const double c2 = 2.0 * CUTOFF_A / g.vs;
-            const long long rx = std::min<long long>(nbx, (long long)((c2 + 3) / 4) + 1), ry = std::min<long long>(nby, (long long)((c2 + 3) / 4) + 1),
+            // tiles (8 x 8 x 8 voxels) one atom can reach: an interval of 2 reach voxels touches at most
+            // floor((2 reach + 7) / 8) + 1 tiles; reach = the cutoff with the list walk's slack
+            const double c2 = 2.0 * CUTOFF_A / g.vs * (1.0 + (double)R_LIST_SLACK);
+            const long long rx = std::min<long long>(g.tiles[0], (long long)((c2 + 7) / 8) + 1),
+                            ry = std::min<long long>(g.tiles[1], (long long)((c2 + 7) / 8) + 1),
                             rz = std::min<long long>(nbz, (long long)((c2 + R_BZ - 1) / R_BZ) + 1);
             nent[b] = (g.atom_end - g.atom_begin) * rx * ry * rz;
             if (rx * ry * rz > L_TABLE_MAX_REACH) list_table = 0;
@@ -1075,7 +1079,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
             ibase.assign((size_t)B + 1, 0);
             long long bsum = 0;
             for (int b = 0; b < B; ++b) {
-                gd[b].tile_base = bsum;  // first 4x4x8 block of this grid (slot index)
+                gd[b].blk_base = bsum;
                 bsum += nblk[b];
                 ibase[b + 1] = ibase[b] + nitem[b];
             }
@@ -1098,14 +1102,15 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         const size_t ni = (size_t)std::max<long long>(items, 1);
         const long long n_words = cdiv(voxels, 32);
         const unsigned fix_cap = (unsigned)std::min<long long>(voxels, 1ll << 22);
-        const size_t nslots = (size_t)run_blocks + 1;  // + 1: the total after the exclusive scan
+        const size_t nslots = (size_t)tiles + 1;  // list slots (tile_base: 8x8x8 tiles) + 1: the total after the exclusive scan
         const long long list_ctas = cdiv(items, L_THREADS);
         if ((rc = scratch_get(h, S_DESC, (size_t)B, &d_grids))) return rc;
         if ((rc = scratch_get(h, S_SORT_PX, ni, &rec_pos))) return rc;
         if ((rc = scratch_get(h, S_SORT_PY, ni, &rec_tag))) return rc;
-        // per block: entries in the CTAs' table segments (blk_count), then the direct insertions (blk_direct)
-        if ((rc = scratch_get(h, S_CELL_COUNT, 2 * nslots, &blk_count))) return rc;
-        unsigned *const blk_direct = blk_count + nslots;
+        // per tile: entries in the CTAs' table segments (blk_count), the direct insertions (blk_direct), the blocks with a
+        // candidate (tile_bits); behind them the compact output's per-block flags
+        if ((rc = scratch_get(h, S_CELL_COUNT, 3 * nslots + (blk_rank ? (size_t)run_blocks + 1 : 0), &blk_count))) return rc;
+        unsigned *const blk_direct = blk_count + nslots, *const tile_bits = blk_direct + nslots, *const blk_flag = tile_bits + nslots;
         if (list_table && list_ctas > 0) {  // the count pass's table segments, read back by the fill pass
             if ((rc = scratch_get(h, S_BLK_SEGS, (size_t)list_ctas * (L_SEG_WORDS + 1), &segs))) return rc;
             seg_n = segs + (size_t)list_ctas * L_SEG_WORDS;
@@ -1123,7 +1128,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         {
             size_t rank_bytes = 0;
             MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, list_len, blk_start, (int)nslots, st));
-            MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, rank_bytes, blk_count, blk_start, (int)nslots, st));
+            MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, rank_bytes, blk_count, blk_start, (int)(run_blocks + 1), st));
             scan_bytes = std::max(scan_bytes, rank_bytes);
             void *tmp = nullptr;
             if ((rc = scratch_get(h, S_SCAN_TMP, scan_bytes, &tmp))) return rc;
@@ -1146,7 +1151,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
             MKB_CUDA(h, cudaMemcpyAsync(d_ibase, static_cast<char *>(stage) + gbytes, ibytes, cudaMemcpyHostToDevice, st));
             MKB_CUDA(h, cudaEventRecord(*sev, st));
         }
-        MKB_CUDA(h, cudaMemsetAsync(blk_count, 0, sizeof(unsigned) * 2 * nslots, st));
+        MKB_CUDA(h, cudaMemsetAsync(blk_count, 0, sizeof(unsigned) * 3 * nslots, st));
         MKB_CUDA(h, cudaMemsetAsync(d_bitmap, 0, sizeof(unsigned) * (size_t)n_words, st));
         MKB_CUDA(h, cudaMemsetAsync(d_queue, 0, sizeof(unsigned) * 64, st));
         MKB_CUDA(h, cudaMemsetAsync(d_fix, 0, sizeof(unsigned long long) * FIX_HDR, st));
@@ -1166,7 +1171,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         h->last_kernel = "occ_fill_runs_kernel";
         if (items > 0) {
             occ_prep_kernel<<<(unsigned)list_ctas, L_THREADS, 0, st>>>(coords, sigmas, radii, chanmask, d_grids, B, items, rec_pos, rec_tag,
-                                                                       blk_count, blk_direct, segs, seg_n, list_table);
+                                                                       blk_count, blk_direct, tile_bits, segs, seg_n, list_table);
             MKB_LAUNCHED(h);
         }
         MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, list_len, blk_start, (int)nslots, st));
@@ -1176,10 +1181,10 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
                                                                            blk_ent, list_table);
             MKB_LAUNCHED(h);
         }
-        if (blk_rank) {  // record index of every non-empty block (the flags overwrite all of blk_count, unused after the scan)
-            occ_blk_flag_kernel<<<(unsigned)cdiv(run_blocks + 1, 256), 256, 0, st>>>(blk_start, run_blocks, blk_count);
+        if (blk_rank) {  // record index of every non-empty block
+            occ_blk_flag_kernel<<<(unsigned)cdiv(run_blocks + 1, 256), 256, 0, st>>>(d_grids, B, tile_bits, run_blocks, blk_flag);
             MKB_LAUNCHED(h);
-            MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, blk_count, blk_rank, (int)(run_blocks + 1), st));
+            MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, blk_flag, blk_rank, (int)(run_blocks + 1), st));
             h->launches++;
             if (host_rank) {  // the block index leaves for the host NOW (side stream), before the fill kernel starts
                 MKB_CUDA(h, cudaEventRecord(h->aux_ev[2], st));
@@ -1192,7 +1197,7 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
         {
             RunParams rp;
             rp.grids = d_grids; rp.B = B;
-            rp.rec_pos = rec_pos; rp.rec_tag = rec_tag; rp.blk_start = blk_start; rp.blk_ent = blk_ent;
+            rp.rec_pos = rec_pos; rp.rec_tag = rec_tag; rp.blk_start = blk_start; rp.tile_bits = tile_bits; rp.blk_ent = blk_ent;
             rp.sigmas = sigmas; rp.out = out;
             rp.item_base = d_ibase; rp.queue = d_queue;
             rp.total_items = (unsigned)run_items;
@@ -1213,7 +1218,8 @@ static int occupancy_grid_batch_impl(mkb_handle_t h, void *stream, const float *
             rp.u_nby = (unsigned)((g0d.dims[1] + 3) / 4);
             rp.u_nzc = (unsigned)(((g0d.dims[2] + R_BZ - 1) / R_BZ + run_zc - 1) / run_zc);
             rp.zc = run_zc;
-            rp.u_bpg = (unsigned)(B > 1 ? gd[1].tile_base - g0d.tile_base : 0);
+            rp.u_bpg = (unsigned)(B > 1 ? gd[1].blk_base - g0d.blk_base : 0);
+            rp.u_tpg = (unsigned)(B > 1 ? gd[1].tile_base - g0d.tile_base : 0);
             if (h->timing) MKB_CUDA(h, cudaEventRecord(h->ev[1], st));
             const unsigned nctas = (unsigned)std::min<long long>((long long)h->sm_count * MKB_R_MIN_CTAS, cdiv((long long)rp.total_items, R_WARPS));
             rp.use_tmap = 0;
