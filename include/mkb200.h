@@ -392,6 +392,27 @@ int mkb_fluctuation(mkb_handle_t h, void *stream, const mkb_traj *t, const uint3
                     const uint32_t *frames, int64_t n_frames, const double *records, const double *centre,
                     const int64_t *group_offsets, int64_t n_groups, float *out, int64_t ld_out);
 
+/* K20: weighted per-frame moments of atom groups, replace the per-frame centres and spreads of MetricGyration
+ * (moleculekit/projections/metricgyration.py) and MetricSphericalCoordinate
+ * (moleculekit/projections/metricsphericalcoordinate.py) after the reference's align.  t, sel, frames and records as for
+ * the K15 entry points above (device pointers; c = the aligned float32 coordinate).  weights [n_sel] float64 and
+ * group_offsets [n_groups + 1] int64 are HOST arrays (they size the launch): group g is the selection positions
+ * [off[g], off[g+1]); the offsets run from 0 to n_sel and increase strictly (no empty group); weights NULL = all 1; a
+ * group whose weights do not sum to a finite value > 0 is MKB_ERR_BAD_ARG.  Every check is made before any work is
+ * enqueued; the call returns once both arrays have been copied.
+ *
+ * out [n][n_groups][6] float64 (device), W the group's weight total:
+ *   out[(k n_groups + g) 6 + d]     = mu_d = sum w c_d / W
+ *   out[(k n_groups + g) 6 + 3 + d] = v_d = sum w (c_d - mu_d)^2 / W, per axis (never negative)
+ * The sums run in float64 relative to the group's first position in the same frame, within segments of at most 512
+ * positions that depend only on the group sizes, added in a fixed order: the bits of a frame's row depend only on the
+ * selection, groups and weights (not on the grid, the frame slice or the rest of the frame list).  A non-finite
+ * coordinate in a group gives NaN in all six values of that (item, group) only.  The handle's timing events bracket the
+ * kernels (main; prep is empty). */
+int mkb_frame_moments(mkb_handle_t h, void *stream, const mkb_traj *t, const uint32_t *sel, int64_t n_sel,
+                      const uint32_t *frames, int64_t n_frames, const double *records, const double *weights,
+                      const int64_t *group_offsets, int64_t n_groups, double *out);
+
 /* K16: torsion angles, replace the per-dihedral loop of MetricDihedral (moleculekit/projections/metricdihedral.py over
  * moleculekit.dihedral.dihedralAngle).  All pointers except the mkb_traj struct are device pointers.  quads [n_quads][4]
  * int32 = atom rows of t (p0, p1, p2, p3 of each dihedral), 16-byte aligned; n_quads == 0 is MKB_ERR_BAD_ARG.  frames

@@ -44,7 +44,7 @@ EXPORTS = [
     "mkb_bonds_count", "mkb_bonds_fill", "mkb_shell_counts", "mkb_wrap_box", "mkb_within_distance", "mkb_xtc_decode",
     "mkb_wrap_triclinic", "mkb_hbonds_count", "mkb_hbonds_fill", "mkb_ring_pairs_count", "mkb_ring_pairs_fill",
     "mkb_align_fit", "mkb_align_apply", "mkb_rmsd", "mkb_coordinates", "mkb_coord_sums", "mkb_fluctuation",
-    "mkb_dihedrals", "mkb_sasa", "mkb_sasa_chunk_frames", "mkb_dssp", "mkb_dssp_chunk_frames",
+    "mkb_frame_moments", "mkb_dihedrals", "mkb_sasa", "mkb_sasa_chunk_frames", "mkb_dssp", "mkb_dssp_chunk_frames",
     "mkb_tmscore", "mkb_tmscore_max_pairs",
 ]
 
@@ -122,6 +122,7 @@ def load():
     lib.mkb_coordinates.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, vp, i64]
     lib.mkb_coord_sums.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, vp]
     lib.mkb_fluctuation.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, vp, vp, i64, vp, i64]
+    lib.mkb_frame_moments.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, vp, vp, i64, vp]
     lib.mkb_dihedrals.argtypes = [vp, vp, tp, vp, i64, vp, i64, i32, vp, i64]
     lib.mkb_sasa.argtypes = [vp, vp, tp, vp, i64, vp, vp, i64, vp, i64, vp, i32, vp, i64, vp, i64, vp]
     lib.mkb_sasa_chunk_frames.argtypes = [i64, i64, i64]

@@ -1,8 +1,9 @@
-"""Aligned coordinate features, frame sums and per-atom fluctuations on the GPU (K15).
+"""Aligned coordinate features, frame sums and per-atom fluctuations (K15), and per-frame group moments (K20) on the GPU.
 
   coordinates_device    (n, 3k) float32 rows: the aligned coordinates of the selection, X block | Y block | Z block
   coord_sums_device     (k, 3) float64 sums over the listed frames (the mean is the sum over the frame count)
   fluctuation_device    (n, k) or (n, G) float32 squared deviations from a centre, per atom or averaged per group
+  frame_moments_device  (n, G, 6) float64 weighted means and per-axis variances of groups of the selection, per frame
 
 CUDA tensors in, stream-ordered, like :func:`moleculekit_b200.align.rmsd_device`: ``coords`` is the (N, 3, F) float32
 frame-minor trajectory (or a frame slice of one), ``sel`` / ``frames`` int32 CUDA tensors (``frames`` None = every
@@ -96,4 +97,34 @@ def fluctuation_device(coords, sel, centre, records=None, frames=None, groups=No
     t = _lib.traj(coords)
     _lib.call(dev, "mkb_fluctuation", C.byref(t), _lib.ptr(sel), k, _lib.ptr(frames), n, _lib.ptr(records),
               _lib.ptr(centre), _lib.ptr(groups), G, _lib.ptr(out), ld)
+    return out
+
+
+def frame_moments_device(coords, sel, records=None, frames=None, weights=None, groups=None):
+    """(n, G, 6) float64 CUDA (K20): per listed frame and group of selection positions, the weighted mean of the aligned
+    float32 coordinate (columns 0-2) and the weighted variance around it per axis (columns 3-5), both over the group's
+    weight total.  ``weights`` (k,) float64 (None = all 1) and ``groups`` (G + 1,) int64 offsets over the selection
+    positions (None = one group of all k) are small host-side arrays -- a CPU tensor, a numpy array or a list; CUDA
+    tensors are copied back.  The library rejects offsets that do not increase strictly from 0 to k and groups whose
+    weights do not sum to a finite value > 0.  The bits of a frame's row depend only on the selection, groups and weights,
+    so repeated calls, a frame slice and the equivalent explicit frame list agree bit for bit."""
+    dev = _lib.tensor_device(coords, "frame_moments_device")
+    _lib.index_arg(sel, dev)
+    _lib.index_arg(frames, dev)
+    k = int(sel.numel())
+    n = coords.shape[2] if frames is None else int(frames.numel())
+    _check_records(records, n)
+    if weights is not None:
+        weights = torch.as_tensor(weights, dtype=torch.float64, device="cpu").contiguous()
+        assert tuple(weights.shape) == (k,), f"weights must be ({k},), got {tuple(weights.shape)}"
+    groups = torch.tensor([0, k]) if groups is None else groups
+    groups = torch.as_tensor(groups, dtype=torch.int64, device="cpu").contiguous()
+    assert groups.ndim == 1, "groups must be 1-D offsets"
+    G = int(groups.numel()) - 1
+    out = torch.empty((n, max(G, 0), 6), dtype=torch.float64, device=dev)
+    if n == 0:
+        return out
+    t = _lib.traj(coords)
+    _lib.call(dev, "mkb_frame_moments", C.byref(t), _lib.ptr(sel), k, _lib.ptr(frames), n, _lib.ptr(records),
+              _lib.ptr(weights), _lib.ptr(groups), G, _lib.ptr(out))
     return out

@@ -46,6 +46,8 @@ enum ScratchSlot {
     S_SASA_AREA,    // K17: per-atom areas before the group sums
     S_DSSP,         // K18: the per-frame arrays of one frame chunk, carved from one allocation
     S_TMSCORE_MASK, // K19: two cut-set bitmasks per resident thread
+    S_MOMENT_TAB,   // K20: segment table, group offsets / totals and weights, uploaded per call
+    S_MOMENT_PART,  // K20: per-(segment, frame) partial moment sums
     S_NSLOTS
 };
 
