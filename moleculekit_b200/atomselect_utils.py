@@ -18,6 +18,16 @@ from . import _lib
 from .distance_utils import _check
 
 
+def as_mask(sel, n: int) -> np.ndarray:
+    """(n,) bool mask of ``sel``, a boolean mask or an index array (either of what ``atomselect`` returns)."""
+    mask = np.asarray(sel)
+    if mask.dtype != bool:
+        m = np.zeros(n, dtype=bool)
+        m[mask] = True
+        mask = m
+    return mask
+
+
 def within_distance_device(coords: torch.Tensor, cutoff: float, sel2: torch.Tensor, sel1: torch.Tensor | None = None,
                            results: torch.Tensor | None = None) -> torch.Tensor:
     """K10 on CUDA tensors: coords (N,3) f32 contiguous, sel2 (source) / sel1 (queries; None = all atoms) int32 index
@@ -61,11 +71,7 @@ def within(mol, cutoff: float, source, exclude_source: bool = False, device=None
     """`within <cutoff> of <source>` (exclude_source: `exwithin`) on frame ``mol.frame``: atomselect.py:231-254.
     ``source`` is a boolean mask or an index array; returns the boolean mask over all atoms."""
     n = int(mol.numAtoms)
-    src = np.asarray(source)
-    if src.dtype != bool:
-        m = np.zeros(n, dtype=bool)
-        m[src] = True
-        src = m
+    src = as_mask(source, n)
     mask = np.zeros(n, dtype=bool)
     if not np.any(src):
         return mask

@@ -10,50 +10,8 @@ from __future__ import annotations
 
 import numpy as np
 
-from .metricrmsd import _nonempty
+from .common import check_sizes, fit, nonempty, reference, selections, upload_wrapped
 from .projection import Projection
-
-
-def _reference(refmol, alnsel):
-    """(refmol copy, its coordinates at refmol.frame as (N, 3, 1) float32, the alignment mask on it)"""
-    ref = refmol.copy()
-    frame = int(getattr(refmol, "frame", 0))
-    coords = np.ascontiguousarray(refmol.coords[:, :, frame:frame + 1], dtype=np.float32)
-    return ref, coords, _nonempty(ref, alnsel, "Reference alignment")
-
-
-def _check_sizes(what, a, b):
-    if int(a.sum()) != int(b.sum()):
-        raise RuntimeError(f"The {what} selections of the trajectory and the reference differ in size: "
-                           f"{int(a.sum())} and {int(b.sum())} atoms.")
-
-
-def _upload_wrap_fit(mol, centersel, pbc, refcoords, trajalnsel, refalnsel, device):
-    """The device pipeline shared by MetricCoordinate and MetricFluctuation: upload ``mol.coords`` once, wrap it around
-    ``centersel`` when ``pbc`` (``wrap_plan(...).run_device``), and with a reference fit every frame's ``trajalnsel``
-    atoms onto its ``refalnsel`` atoms (``LinAlgError`` on a non-finite fit, before anything else is computed).
-    Returns (the (N, 3, F) CUDA tensor, the fit records or None)."""
-    import torch
-
-    from ..align import raise_if_nonfinite, superpose_device
-    from .. import _lib
-    from ..wrapping import wrap_plan
-
-    dev = _lib.device(device)
-    d = torch.from_numpy(np.ascontiguousarray(mol.coords, dtype=np.float32)).to(dev)
-    if pbc:
-        plan = wrap_plan(mol, centersel)
-        if plan is not None:
-            plan.run_device(d, torch.from_numpy(np.ascontiguousarray(mol.box, dtype=np.float32)).to(dev))
-    if refcoords is None:
-        return d, None
-
-    def idx(mask):
-        return torch.from_numpy(np.where(mask)[0].astype(np.int32)).to(dev)
-
-    records, status = superpose_device(d, idx(trajalnsel), torch.from_numpy(refcoords).to(dev), idx(refalnsel))
-    raise_if_nonfinite(status, np.arange(d.shape[2]))
-    return d, records
 
 
 class MetricCoordinate(Projection):
@@ -81,21 +39,16 @@ class MetricCoordinate(Projection):
                 trajalnsel = "protein and name CA"
             if refalnsel is None:
                 refalnsel = trajalnsel
-            self._refmol, self._refcoords, self._refalnsel = _reference(refmol, refalnsel)
+            self._refmol, self._refcoords = reference(refmol)
+            self._refalnsel = nonempty(self._refmol, refalnsel, "Reference alignment")
         self._atomsel, self._trajalnsel, self._centersel = atomsel, trajalnsel, centersel
         self._pbc = pbc
         self.device = None  # CUDA device for project(); None = current device
 
     def _calculateMolProp(self, mol, props="all"):
-        props = ("atomsel", "trajalnsel", "centersel") if props == "all" else props
-        res = {}
-        if "atomsel" in props:
-            res["atomsel"] = _nonempty(mol, self._atomsel, "Atom")
-        if "trajalnsel" in props and self._refmol is not None:
-            res["trajalnsel"] = _nonempty(mol, self._trajalnsel, "Alignment")
-        if "centersel" in props and self._pbc:
-            res["centersel"] = _nonempty(mol, self._centersel, "Centering")
-        return res
+        return selections(mol, props, (("atomsel", self._atomsel, "Atom", True),
+                                       ("trajalnsel", self._trajalnsel, "Alignment", self._refmol is not None),
+                                       ("centersel", self._centersel, "Centering", self._pbc)))
 
     def project(self, mol) -> np.ndarray:
         """(numFrames, 3n) float32 aligned coordinates."""
@@ -106,12 +59,12 @@ class MetricCoordinate(Projection):
         props = self._getMolProp(mol, "all")
         sel = np.where(props["atomsel"])[0]
         if self._refmol is not None:
-            _check_sizes("alignment", props["trajalnsel"], self._refalnsel)
+            check_sizes("alignment", props["trajalnsel"], self._refalnsel)
         F = mol.coords.shape[2]
         if F == 0:
             return np.zeros((0, 3 * sel.size), np.float32)
-        d, records = _upload_wrap_fit(mol, props.get("centersel"), self._pbc, self._refcoords, props.get("trajalnsel"),
-                                      self._refalnsel, self.device)
+        d = upload_wrapped(mol, props.get("centersel"), self.device)
+        records = None if self._refmol is None else fit(d, props["trajalnsel"], self._refcoords, self._refalnsel)
         d_sel = torch.from_numpy(sel.astype(np.int32)).to(d.device)
         return coordinates_device(d, d_sel, records).cpu().numpy()
 

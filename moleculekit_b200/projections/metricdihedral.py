@@ -10,7 +10,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from .metricrmsd import _nonempty
+from .common import column, nonempty, residues
 from .projection import Projection
 
 # (residue offset, atom name) of the four atoms; offset -1 = the previous residue, +1 = the next one
@@ -53,27 +53,6 @@ def _check_types(dih):
         raise ValueError(f"Unknown dihedral type(s) {bad}; supported: {', '.join(TYPES)}")
 
 
-def _column(mol, field, default):
-    v = getattr(mol, field, None)
-    return np.full(mol.numAtoms, default, dtype=object) if v is None else np.asarray(v)
-
-
-def residues(mol, sel):
-    """The residues of the ``sel`` atoms in atom order: a new residue starts wherever resid, insertion, chain or segid
-    changes from one selected atom to the next.  Returns a list of atom index arrays."""
-    idx = np.where(sel)[0]
-    if idx.size == 0:
-        return []
-    keys = [np.asarray(_column(mol, f, d))[idx] for f, d in (("resid", 0), ("insertion", ""), ("chain", ""),
-                                                            ("segid", ""))]
-    change = np.zeros(idx.size, dtype=bool)
-    change[0] = True
-    for k in keys:
-        change[1:] |= k[1:] != k[:-1]
-    starts = np.append(np.where(change)[0], idx.size)
-    return [idx[a:b] for a, b in zip(starts[:-1], starts[1:])]
-
-
 def select_dihedrals(mol, sel, dih):
     """(quads (m, 4) int64 atom indices, labels [(type, residue's first atom)]) of the ``dih`` torsions of the ``sel``
     residues, residue by residue and, within a residue, in the order of ``dih``.  A torsion is skipped when one of its
@@ -81,8 +60,8 @@ def select_dihedrals(mol, sel, dih):
     segid."""
     _check_types(dih)
     res = residues(mol, sel)
-    name, resname = _column(mol, "name", ""), _column(mol, "resname", "")
-    chain, segid = _column(mol, "chain", ""), _column(mol, "segid", "")
+    name, resname = column(mol, "name", ""), column(mol, "resname", "")
+    chain, segid = column(mol, "chain", ""), column(mol, "segid", "")
     lookup = []
     for atoms in res:
         names = {}
@@ -169,7 +148,7 @@ class MetricDihedral(Projection):
         props = ("dihedrals",) if props == "all" else props
         res = {}
         if "dihedrals" in props:
-            res["dihedrals"] = select_dihedrals(mol, _nonempty(mol, self._protsel, "Protein"), self._dih)
+            res["dihedrals"] = select_dihedrals(mol, nonempty(mol, self._protsel, "Protein"), self._dih)
         return res
 
     def project(self, mol) -> np.ndarray:
@@ -194,7 +173,7 @@ class MetricDihedral(Projection):
         from pandas import DataFrame
 
         quads, labels = self._getMolProp(mol, "dihedrals")
-        resname, resid = _column(mol, "resname", ""), _column(mol, "resid", 0)
+        resname, resid = column(mol, "resname", ""), column(mol, "resid", 0)
         kinds = ("Sine", "Cosine") if self._sincos else ("Angle",)
         types, indexes, desc = [], [], []
         for q, (d, a) in zip(quads, labels):

@@ -1,7 +1,7 @@
 """Drop-in for ``moleculekit.projections.metricfluctuation.MetricFluctuation``: per-atom (or per-residue) squared
 deviation of every frame from the mean structure or from a reference -- what an RMSF is computed from.
 
-``project`` runs MetricCoordinate's device pipeline (one upload, wrap, fit) and then, without a reference, the frame
+``project`` runs the shared pipeline of ``common`` (one upload, wrap, fit) and then, without a reference, the frame
 sums of the selection (K15, a fixed-order float64 reduction) for the mean, and the squared deviations straight from the
 trajectory (K15): the (numFrames, 3n) coordinate matrix is never materialised, and only the result comes back.
 Frames are not independent without a reference (the mean spans all of them): shard such a projection with
@@ -11,8 +11,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from .metriccoordinate import _check_sizes, _reference, _upload_wrap_fit
-from .metricrmsd import _nonempty
+from .common import check_sizes, fit, nonempty, reference, selections, upload_wrapped
 from .projection import Projection
 
 
@@ -57,23 +56,18 @@ class MetricFluctuation(Projection):
             refalnstr = trajalnstr
         self._refmol = self._refcoords = self._refalnsel = self._refatomsel = None
         if refmol is not None:
-            self._refmol, self._refcoords, self._refalnsel = _reference(refmol, refalnstr)
-            self._refatomsel = _nonempty(self._refmol, atomsel, "Reference atom")
+            self._refmol, self._refcoords = reference(refmol)
+            self._refalnsel = nonempty(self._refmol, refalnstr, "Reference alignment")
+            self._refatomsel = nonempty(self._refmol, atomsel, "Reference atom")
         self._atomsel, self._trajalnsel, self._centersel = atomsel, trajalnstr, centerstr
         self._pbc = pbc
         self._mode = mode
         self.device = None  # CUDA device for project(); None = current device
 
     def _calculateMolProp(self, mol, props="all"):
-        props = ("atomsel", "trajalnsel", "centersel") if props == "all" else props
-        res = {}
-        if "atomsel" in props:
-            res["atomsel"] = _nonempty(mol, self._atomsel, "Atom")
-        if "trajalnsel" in props and self._refmol is not None:
-            res["trajalnsel"] = _nonempty(mol, self._trajalnsel, "Alignment")
-        if "centersel" in props and self._pbc:
-            res["centersel"] = _nonempty(mol, self._centersel, "Centering")
-        return res
+        return selections(mol, props, (("atomsel", self._atomsel, "Atom", True),
+                                       ("trajalnsel", self._trajalnsel, "Alignment", self._refmol is not None),
+                                       ("centersel", self._centersel, "Centering", self._pbc)))
 
     def _layout(self, mol):
         """(selected atoms in output order (int64), group offsets or None): residue mode orders the selection by resid."""
@@ -87,12 +81,10 @@ class MetricFluctuation(Projection):
         """(n, 3) float64: the reference's ``atomsel`` atoms in the output order of :meth:`_layout` (None without one)."""
         if self._refmol is None:
             return None
-        idx = np.where(self._getMolProp(mol, "atomsel"))[0]
-        ref = np.where(self._refatomsel)[0]
-        if idx.size != ref.size:
-            raise RuntimeError(f"The atom selections of the trajectory and the reference differ in size: {idx.size} and "
-                               f"{ref.size} atoms.")
-        rc = self._refcoords[ref, :, 0].astype(np.float64)
+        atomsel = self._getMolProp(mol, "atomsel")
+        check_sizes("atom", atomsel, self._refatomsel)
+        idx = np.where(atomsel)[0]
+        rc = self._refcoords[np.where(self._refatomsel)[0], :, 0].astype(np.float64)
         if self._mode == "residue":
             rc = rc[residue_groups(np.asarray(mol.resid)[idx])[0]]
         return np.ascontiguousarray(rc)
@@ -103,11 +95,11 @@ class MetricFluctuation(Projection):
 
         props = self._getMolProp(mol, "all")
         if self._refmol is not None:
-            _check_sizes("alignment", props["trajalnsel"], self._refalnsel)
+            check_sizes("alignment", props["trajalnsel"], self._refalnsel)
             self.reference_centre(mol)
         sel, offsets = self._layout(mol)
-        d, records = _upload_wrap_fit(mol, props.get("centersel"), self._pbc, self._refcoords,
-                                      props.get("trajalnsel"), self._refalnsel, self.device)
+        d = upload_wrapped(mol, props.get("centersel"), self.device)
+        records = None if self._refmol is None else fit(d, props["trajalnsel"], self._refcoords, self._refalnsel)
         d_sel = torch.from_numpy(sel.astype(np.int32)).to(d.device)
         d_off = None if offsets is None else torch.from_numpy(offsets).to(d.device)
         return d, records, d_sel, d_off

@@ -1,7 +1,7 @@
 """Drop-in for ``moleculekit.projections.metricgyration.MetricGyration``: the mass-weighted radius of gyration of a
 selection per frame, with its per-axis components.
 
-``project`` runs MetricCoordinate's device pipeline (one upload, wrap, optional fit) and then one K20 call, the
+``project`` runs the shared pipeline of ``common`` (one upload, wrap, optional fit) and then one K20 call, the
 mass-weighted centre and per-axis spread of the selection in every frame: the aligned trajectory is never written and
 only six float64 values per frame come back.  ``mol`` is duck-typed (a moleculekit ``Molecule`` or
 :class:`moleculekit_b200.molecule_lite.MolLite`) and is not modified.
@@ -10,8 +10,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from .metriccoordinate import _check_sizes, _reference, _upload_wrap_fit
-from .metricrmsd import _nonempty
+from .common import check_sizes, fit, nonempty, reference, selections, upload_wrapped
 from .projection import Projection
 
 
@@ -65,21 +64,16 @@ class MetricGyration(Projection):
             refalnstr = trajalnstr
         self._refmol = self._refcoords = self._refalnsel = None
         if refmol is not None:
-            self._refmol, self._refcoords, self._refalnsel = _reference(refmol, refalnstr)
+            self._refmol, self._refcoords = reference(refmol)
+            self._refalnsel = nonempty(self._refmol, refalnstr, "Reference alignment")
         self._atomsel, self._trajalnsel, self._centersel = atomsel, trajalnstr, centerstr
         self._pbc = pbc
         self.device = None  # CUDA device for project(); None = current device
 
     def _calculateMolProp(self, mol, props="all"):
-        props = ("atomsel", "trajalnsel", "centersel") if props == "all" else props
-        res = {}
-        if "atomsel" in props:
-            res["atomsel"] = _nonempty(mol, self._atomsel, "Atom")
-        if "trajalnsel" in props and self._refmol is not None:
-            res["trajalnsel"] = _nonempty(mol, self._trajalnsel, "Alignment")
-        if "centersel" in props and self._pbc:
-            res["centersel"] = _nonempty(mol, self._centersel, "Centering")
-        return res
+        return selections(mol, props, (("atomsel", self._atomsel, "Atom", True),
+                                       ("trajalnsel", self._trajalnsel, "Alignment", self._refmol is not None),
+                                       ("centersel", self._centersel, "Centering", self._pbc)))
 
     def project(self, mol) -> np.ndarray:
         """(numFrames, 4) float32 ``[rg, rg_x, rg_y, rg_z]``."""
@@ -89,13 +83,13 @@ class MetricGyration(Projection):
 
         props = self._getMolProp(mol, "all")
         if self._refmol is not None:
-            _check_sizes("alignment", props["trajalnsel"], self._refalnsel)
+            check_sizes("alignment", props["trajalnsel"], self._refalnsel)
         sel = np.where(props["atomsel"])[0]
         masses = selection_masses(mol, sel)
         if mol.coords.shape[2] == 0:
             return np.zeros((0, 4), np.float32)
-        d, records = _upload_wrap_fit(mol, props.get("centersel"), self._pbc, self._refcoords, props.get("trajalnsel"),
-                                      self._refalnsel, self.device)
+        d = upload_wrapped(mol, props.get("centersel"), self.device)
+        records = None if self._refmol is None else fit(d, props["trajalnsel"], self._refcoords, self._refalnsel)
         d_sel = torch.from_numpy(sel.astype(np.int32)).to(d.device)
         moments = frame_moments_device(d, d_sel, records, weights=masses)
         return gyration_features(moments[:, 0].cpu().numpy())

@@ -14,20 +14,10 @@ import logging
 
 import numpy as np
 
+from .common import check_sizes, device_indices, fit, nonempty, reference, selections, upload_wrapped
 from .projection import Projection
 
 logger = logging.getLogger(__name__)
-
-
-def _nonempty(mol, sel, what):
-    mask = np.asarray(mol.atomselect(sel))
-    if mask.dtype != bool:
-        m = np.zeros(mol.numAtoms, dtype=bool)
-        m[mask] = True
-        mask = m
-    if not mask.any():
-        raise RuntimeError(f"{what} selection resulted in 0 atoms.")
-    return mask
 
 
 class MetricRmsd(Projection):
@@ -43,60 +33,37 @@ class MetricRmsd(Projection):
             refalnstr = trajalnstr
         if refrmsdstr is None:
             refrmsdstr = trajrmsdstr
-        self._refmol = refmol.copy()
-        frame = int(getattr(refmol, "frame", 0))
-        if self._refmol.coords.shape[2] > 1:
-            logger.warning(f"Reference molecule contains multiple frames. MetricRmsd will use frame {frame} as reference.")
-        self._refcoords = np.ascontiguousarray(refmol.coords[:, :, frame:frame + 1], dtype=np.float32)
-        self._refalnsel = _nonempty(self._refmol, refalnstr, "Reference alignment")
-        self._refrmsdsel = _nonempty(self._refmol, refrmsdstr, "Reference RMSD")
+        self._refmol, self._refcoords = reference(refmol, logger, "MetricRmsd")
+        self._refalnsel = nonempty(self._refmol, refalnstr, "Reference alignment")
+        self._refrmsdsel = nonempty(self._refmol, refrmsdstr, "Reference RMSD")
         self._trajalnsel, self._trajrmsdsel = trajalnstr, trajrmsdstr
         self._centersel = centerstr
         self._pbc = pbc
         self.device = None  # CUDA device for project(); None = current device
 
     def _calculateMolProp(self, mol, props="all"):
-        props = ("trajalnsel", "trajrmsdsel", "centersel") if props == "all" else props
-        res = {}
-        if "trajalnsel" in props:
-            res["trajalnsel"] = _nonempty(mol, self._trajalnsel, "Alignment")
-        if "trajrmsdsel" in props:
-            res["trajrmsdsel"] = _nonempty(mol, self._trajrmsdsel, "RMSD atom")
-        if "centersel" in props and self._pbc:
-            res["centersel"] = _nonempty(mol, self._centersel, "Centering")
-        return res
+        return selections(mol, props, (("trajalnsel", self._trajalnsel, "Alignment", True),
+                                       ("trajrmsdsel", self._trajrmsdsel, "RMSD atom", True),
+                                       ("centersel", self._centersel, "Centering", self._pbc)))
 
     def project(self, mol) -> np.ndarray:
         """(numFrames,) float32 RMSDs."""
         import torch
 
-        from ..align import raise_if_nonfinite, rmsd_device, superpose_device
-        from .. import _lib
-        from ..wrapping import wrap_plan
+        from ..align import rmsd_device
 
         props = self._getMolProp(mol, "all")
         aln, rms = props["trajalnsel"], props["trajrmsdsel"]
-        for what, a, b in (("alignment", aln, self._refalnsel), ("RMSD", rms, self._refrmsdsel)):
-            if a.sum() != b.sum():
-                raise RuntimeError(f"The {what} selections of the trajectory and the reference differ in size: "
-                                   f"{int(a.sum())} and {int(b.sum())} atoms.")
+        check_sizes("alignment", aln, self._refalnsel)
+        check_sizes("RMSD", rms, self._refrmsdsel)
         F = mol.coords.shape[2]
         if F == 0:
             return np.zeros(0, np.float32)
-        dev = _lib.device(self.device)
-        d = torch.from_numpy(np.ascontiguousarray(mol.coords, dtype=np.float32)).to(dev)
-        if self._pbc:
-            plan = wrap_plan(mol, props["centersel"])
-            if plan is not None:
-                plan.run_device(d, torch.from_numpy(np.ascontiguousarray(mol.box, dtype=np.float32)).to(dev))
-        ref = torch.from_numpy(self._refcoords).to(dev)
-
-        def idx(mask):
-            return torch.from_numpy(np.where(mask)[0].astype(np.int32)).to(dev)
-
-        records, status = superpose_device(d, idx(aln), ref, idx(self._refalnsel))
-        raise_if_nonfinite(status, np.arange(F))
-        return rmsd_device(d, idx(rms), ref, idx(self._refrmsdsel), records).cpu().numpy()
+        d = upload_wrapped(mol, props.get("centersel"), self.device)
+        ref = torch.from_numpy(self._refcoords).to(d.device)
+        records = fit(d, aln, ref, self._refalnsel)
+        return rmsd_device(d, device_indices(rms, d.device), ref, device_indices(self._refrmsdsel, d.device),
+                           records).cpu().numpy()
 
     def getMapping(self, mol):
         from pandas import DataFrame

@@ -8,8 +8,8 @@ from __future__ import annotations
 
 import numpy as np
 
-from .metricdihedral import _column, residues
-from .metricrmsd import _nonempty
+from ..atomselect_utils import as_mask
+from .common import column, nonempty, residues
 from .projection import Projection
 
 
@@ -24,7 +24,7 @@ class MetricSasa(Projection):
     - ``mode="atom"``: one column per ``sel`` atom, in atom order.  ``mode="residue"``: one column per residue of the
       ``filtersel`` atoms that contains a ``sel`` atom; the column is the float32 sum, in atom order, of the areas of
       every ``filtersel`` atom of the residue.  Residues are runs of consecutive atoms with the same resid, insertion
-      code, chain and segid (:func:`moleculekit_b200.projections.metricdihedral.residues`).
+      code, chain and segid (:func:`moleculekit_b200.projections.common.residues`).
     - Every value is bit-identical to the reference's float32 arithmetic: the area is a count of accessible points.
     - No wrapping and no minimum image.  An atom with a non-finite coordinate takes part in no neighbour relation: its
       own area is that of the full sphere, and it buries no point of another atom.
@@ -60,16 +60,12 @@ class MetricSasa(Projection):
         res = {}
         if "sasa" not in props:
             return res
-        sel = _nonempty(mol, self._sel, "Atom")
-        filt = np.asarray(mol.atomselect(self._filtersel))
-        if filt.dtype != bool:
-            m = np.zeros(mol.numAtoms, bool)
-            m[filt] = True
-            filt = m
+        sel = nonempty(mol, self._sel, "Atom")
+        filt = as_mask(mol.atomselect(self._filtersel), mol.numAtoms)
         if (sel & ~filt).any():
             raise ValueError(f"{int((sel & ~filt).sum())} sel atom(s) lie outside filtersel; their area is undefined")
         env = np.where(filt)[0]
-        radii = sasa_radii(_column(mol, "element", "")[env], self._probe)
+        radii = sasa_radii(column(mol, "element", "")[env], self._probe)
         pos = np.full(mol.numAtoms, -1, np.int64)
         pos[env] = np.arange(env.size)
         if self._mode == "atom":
@@ -110,7 +106,7 @@ class MetricSasa(Projection):
         from pandas import DataFrame
 
         _, _, _, _, cols = self._getMolProp(mol, "sasa")
-        resname, resid, name = _column(mol, "resname", ""), _column(mol, "resid", 0), _column(mol, "name", "")
+        resname, resid, name = column(mol, "resname", ""), column(mol, "resid", 0), column(mol, "name", "")
         if self._mode == "atom":
             desc = [f"SASA of {resname[c[0]]} {resid[c[0]]} {name[c[0]]}" for c in cols]
         else:

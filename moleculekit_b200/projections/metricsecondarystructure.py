@@ -9,8 +9,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from .metricdihedral import _column, residues
-from .metricrmsd import _nonempty
+from .common import column, nonempty, residues
 from .projection import Projection
 
 BACKBONE_NAMES = ("N", "CA", "C", "O")
@@ -19,14 +18,14 @@ BACKBONE_NAMES = ("N", "CA", "C", "O")
 def dssp_residues(mol, sel):
     """(backbone (n, 4) int64 atom indices of N, CA, C, O, flags (n,) uint8, position (ncols,) int64 of every ``sel``
     residue in the DSSP sequence or -1, residue atom lists) of the ``sel`` residues
-    (:func:`moleculekit_b200.projections.metricdihedral.residues`).  A residue enters the sequence when it has atoms
+    (:func:`moleculekit_b200.projections.common.residues`).  A residue enters the sequence when it has atoms
     named N, CA, C and O (the first atom of a repeated name); flag bit 0 marks resname PRO, bit 1 a residue whose chain
     or segid differs from the previous residue of the sequence."""
     from ..dssp import FLAG_CHAIN_START, FLAG_PRO
 
     res = residues(mol, sel)
-    name, resname = _column(mol, "name", ""), _column(mol, "resname", "")
-    chain, segid = _column(mol, "chain", ""), _column(mol, "segid", "")
+    name, resname = column(mol, "name", ""), column(mol, "resname", "")
+    chain, segid = column(mol, "chain", ""), column(mol, "segid", "")
     backbone, flags, pos = [], [], np.full(len(res), -1, np.int64)
     prev = None
     for r, atoms in enumerate(res):
@@ -97,7 +96,7 @@ class MetricSecondaryStructure(Projection):
         props = ("dssp",) if props == "all" else props
         res = {}
         if "dssp" in props:
-            res["dssp"] = dssp_residues(mol, _nonempty(mol, self._sel, "Atom"))
+            res["dssp"] = dssp_residues(mol, nonempty(mol, self._sel, "Atom"))
         return res
 
     def _encode(self, codes, pos):
@@ -138,7 +137,7 @@ class MetricSecondaryStructure(Projection):
         from pandas import DataFrame
 
         _, _, _, cols = self._getMolProp(mol, "dssp")
-        resname, resid = _column(mol, "resname", ""), _column(mol, "resid", 0)
+        resname, resid = column(mol, "resname", ""), column(mol, "resid", 0)
         desc = [f"Secondary structure of residue {resname[c[0]]} {resid[c[0]]}" for c in cols]
         return DataFrame({"type": ["secondary structure"] * len(cols), "atomIndexes": [c.copy() for c in cols],
                           "description": desc})

@@ -1,7 +1,7 @@
 """Drop-in for ``moleculekit.projections.metricsphericalcoordinate.MetricSphericalCoordinate``: the spherical
 coordinates of one selection's centre relative to another's, per frame, after superposition onto a reference.
 
-``project`` runs MetricCoordinate's device pipeline (one upload, wrap, fit) and then one K20 call with two unweighted
+``project`` runs the shared pipeline of ``common`` (one upload, wrap, fit) and then one K20 call with two unweighted
 groups, the reference atoms and the target atoms: only their two centres per frame come back.  ``mol`` is duck-typed
 (a moleculekit ``Molecule`` or :class:`moleculekit_b200.molecule_lite.MolLite`) and is not modified.
 """
@@ -9,8 +9,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from .metriccoordinate import _check_sizes, _reference, _upload_wrap_fit
-from .metricrmsd import _nonempty
+from .common import check_sizes, fit, nonempty, reference, selections, upload_wrapped
 from .projection import Projection
 
 
@@ -53,24 +52,18 @@ class MetricSphericalCoordinate(Projection):
             raise ValueError("MetricSphericalCoordinate needs refmol: every frame is superposed onto it")
         if refalnstr is None:
             refalnstr = trajalnstr
-        self._refmol, self._refcoords, self._refalnsel = _reference(refmol, refalnstr)
+        self._refmol, self._refcoords = reference(refmol)
+        self._refalnsel = nonempty(self._refmol, refalnstr, "Reference alignment")
         self._targetcom, self._refcom = targetcom, refcom
         self._trajalnsel, self._centersel = trajalnstr, centerstr
         self._pbc = pbc
         self.device = None  # CUDA device for project(); None = current device
 
     def _calculateMolProp(self, mol, props="all"):
-        props = ("targetcom", "refcom", "trajalnsel", "centersel") if props == "all" else props
-        res = {}
-        if "targetcom" in props:
-            res["targetcom"] = _nonempty(mol, self._targetcom, "Target COM")
-        if "refcom" in props:
-            res["refcom"] = _nonempty(mol, self._refcom, "Reference COM")
-        if "trajalnsel" in props:
-            res["trajalnsel"] = _nonempty(mol, self._trajalnsel, "Alignment")
-        if "centersel" in props and self._pbc:
-            res["centersel"] = _nonempty(mol, self._centersel, "Centering")
-        return res
+        return selections(mol, props, (("targetcom", self._targetcom, "Target COM", True),
+                                       ("refcom", self._refcom, "Reference COM", True),
+                                       ("trajalnsel", self._trajalnsel, "Alignment", True),
+                                       ("centersel", self._centersel, "Centering", self._pbc)))
 
     def _layout(self, props):
         """(selection: the refcom atoms then the targetcom atoms, group offsets [0, n_ref, n_ref + n_target])"""
@@ -84,12 +77,12 @@ class MetricSphericalCoordinate(Projection):
         from ..coords import frame_moments_device
 
         props = self._getMolProp(mol, "all")
-        _check_sizes("alignment", props["trajalnsel"], self._refalnsel)
+        check_sizes("alignment", props["trajalnsel"], self._refalnsel)
         sel, offsets = self._layout(props)
         if mol.coords.shape[2] == 0:
             return np.zeros((0, 3), np.float32)
-        d, records = _upload_wrap_fit(mol, props.get("centersel"), self._pbc, self._refcoords, props["trajalnsel"],
-                                      self._refalnsel, self.device)
+        d = upload_wrapped(mol, props.get("centersel"), self.device)
+        records = fit(d, props["trajalnsel"], self._refcoords, self._refalnsel)
         d_sel = torch.from_numpy(sel.astype(np.int32)).to(d.device)
         moments = frame_moments_device(d, d_sel, records, groups=offsets)
         return spherical_features(moments.cpu().numpy())

@@ -11,7 +11,7 @@ import logging
 
 import numpy as np
 
-from .metricrmsd import _nonempty
+from .common import nonempty, reference, upload_wrapped
 from .projection import Projection
 
 logger = logging.getLogger(__name__)
@@ -55,13 +55,9 @@ class MetricTMscore(Projection):
         super().__init__()
         if reftmstr is None:
             reftmstr = trajtmstr
-        self._refmol = refmol.copy()
-        frame = int(getattr(refmol, "frame", 0))
-        if self._refmol.coords.shape[2] > 1:
-            logger.warning(f"Reference molecule contains multiple frames. MetricTMscore will use frame {frame} as "
-                           "reference.")
+        self._refmol, refcoords = reference(refmol, logger, "MetricTMscore")
         self._refca = ca_atoms(self._refmol, reftmstr, "Reference TM-score")
-        self._refcoords = np.ascontiguousarray(refmol.coords[self._refca][:, :, frame:frame + 1], dtype=np.float32)
+        self._refcoords = refcoords[self._refca]
         self._trajtmsel = trajtmstr
         self._centersel = centerstr
         self._pbc = pbc
@@ -75,28 +71,22 @@ class MetricTMscore(Projection):
         if "trajca" in props:
             res["trajca"] = ca_atoms(mol, self._trajtmsel, "TM-score")
         if "centersel" in props and self._pbc:
-            res["centersel"] = _nonempty(mol, self._centersel, "Centering")
+            res["centersel"] = nonempty(mol, self._centersel, "Centering")
         return res
 
     def project(self, mol) -> np.ndarray:
         """(numFrames,) float32 TM-scores."""
         import torch
 
-        from .. import _lib
         from ..tmscore import tmscore_device
-        from ..wrapping import wrap_plan
 
         props = self._getMolProp(mol, "all")
         ca = props["trajca"]
         F = mol.coords.shape[2]
         if F == 0:
             return np.zeros(0, np.float32)
-        dev = _lib.device(self.device)
-        d = torch.from_numpy(np.ascontiguousarray(mol.coords, dtype=np.float32)).to(dev)
-        if self._pbc:
-            plan = wrap_plan(mol, props["centersel"])
-            if plan is not None:
-                plan.run_device(d, torch.from_numpy(np.ascontiguousarray(mol.box, dtype=np.float32)).to(dev))
+        d = upload_wrapped(mol, props.get("centersel"), self.device)
+        dev = d.device
         ref = torch.from_numpy(self._refcoords).to(dev)
         sel = torch.from_numpy(ca.astype(np.int32)).to(dev)
         refsel = torch.arange(self._refca.size, dtype=torch.int32, device=dev)

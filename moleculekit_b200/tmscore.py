@@ -19,6 +19,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .atomselect_utils import as_mask
 
 
 def tm_parameters(L: int, lnorm: int):
@@ -47,11 +48,7 @@ def max_pairs() -> int:
 
 def ca_atoms(mol, sel, what: str) -> np.ndarray:
     """int64 indices of the atoms of ``sel`` named CA, ascending; RuntimeError when there are none."""
-    mask = np.asarray(mol.atomselect(sel))
-    if mask.dtype != bool:
-        m = np.zeros(mol.numAtoms, dtype=bool)
-        m[mask] = True
-        mask = m
+    mask = as_mask(mol.atomselect(sel), mol.numAtoms)
     idx = np.where(mask & (np.asarray(mol.name).astype(str) == "CA"))[0]
     if idx.size == 0:
         raise RuntimeError(f"{what} selection resulted in 0 CA atoms.")

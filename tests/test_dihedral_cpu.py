@@ -109,7 +109,8 @@ def _per_type(mol, quads, labels):
 
 @pytest.mark.parametrize("which", ["3ptb", "traj20"])
 def test_selection_counts(which, g_3ptb, g_traj):
-    from moleculekit_b200.projections.metricdihedral import ALIASES, CHI, residues, select_dihedrals
+    from moleculekit_b200.projections.common import residues
+    from moleculekit_b200.projections.metricdihedral import ALIASES, CHI, select_dihedrals
 
     g = g_3ptb if which == "3ptb" else g_traj
     mol = _lite(g)
@@ -143,7 +144,8 @@ def test_selection_counts(which, g_3ptb, g_traj):
 
 
 def test_ends_and_chain_breaks(g_3ptb):
-    from moleculekit_b200.projections.metricdihedral import residues, select_dihedrals
+    from moleculekit_b200.projections.common import residues
+    from moleculekit_b200.projections.metricdihedral import select_dihedrals
 
     mol = _lite(g_3ptb)
     prot = mol.atomselect("protein")

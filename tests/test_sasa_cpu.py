@@ -87,7 +87,7 @@ def _lite(g, **kw):
 
 
 def test_columns_and_mapping(g_3ptb):
-    from moleculekit_b200.projections.metricdihedral import residues
+    from moleculekit_b200.projections.common import residues
     from moleculekit_b200.projections.metricsasa import MetricSasa
 
     mol = _lite(g_3ptb)
