@@ -259,6 +259,34 @@ typedef struct {
 int mkb_xtc_decode(mkb_handle_t h, void *stream, const uint8_t *file_bytes, int64_t file_size, const mkb_xtc_frame *frames,
                    int64_t n_frames, int64_t natoms, float *coords, int64_t frame_stride, float scale, int32_t *status);
 
+/* K21: XTC compressed coordinates written on the device, the inverse of K11; replaces xdrfile_compress_coord_float
+ * (src/xdrfile.cpp) inside the frame loop of the reference's write_xtc.  coords float32 device, element (a, d, f) at
+ * coords[(a*3 + d)*frame_stride + f]; every value is first multiplied by `scale` as a float32 operation of its own (1 = the
+ * input is in nm, 0.1 = Angstrom in; skipped when scale == 1), then taken to the lattice at `precision` (<= 0 or NaN means
+ * 1000) with the reference's individually rounded float32 steps.  Frame f's coordinate block -- what follows the second
+ * atom count of its frame header in the file -- is written at out_bytes + frame_offsets[f], frame_nbytes[f] bytes long:
+ *     natoms > 9:   precision (float), minint[3], maxint[3], smallidx, byte count of the bit stream (all 32-bit big-endian),
+ *                   then the bit stream zero-padded to a multiple of 4 bytes
+ *     natoms <= 9:  3*natoms big-endian floats
+ * Blocks are packed back to back in frame order; every length is a multiple of 4 and out_bytes must be 4-byte aligned.
+ * frame_offsets [n_frames + 1] int64, frame_nbytes [n_frames] int32 and status [n_frames] int32 are device arrays;
+ * frame_offsets[n_frames] is the total.  A frame whose status is not 0 takes no bytes:
+ *     MKB_XTC_ENC_COORD_OVERFLOW   a lattice coordinate beyond INT_MAX - 2 (or a coordinate that is not a number)
+ *     MKB_XTC_ENC_RANGE_OVERFLOW   the lattice range of an axis reaches INT_MAX - 2
+ *     (both are the reference's "Internal overflow compressing coordinates")
+ *     MKB_XTC_ENC_SMALLIDX_RANGE   consecutive atoms so far apart that the reference would read past its table of ranges
+ * The lengths are known only after a first pass over the frames, so this call synchronises the stream once (as
+ * mkb_contacts_count does).  When the blocks need more than out_capacity bytes nothing is written to out_bytes and the
+ * call returns MKB_ERR_CAPACITY with the three tables filled: frame_offsets[n_frames] is the capacity to come back with
+ * (out_bytes may be NULL when out_capacity is 0).  n_frames == 0 or natoms == 0 returns MKB_OK and touches nothing.
+ * Byte-identical to the reference writer. */
+#define MKB_XTC_ENC_COORD_OVERFLOW (-1)
+#define MKB_XTC_ENC_RANGE_OVERFLOW (-2)
+#define MKB_XTC_ENC_SMALLIDX_RANGE (-3)
+int mkb_xtc_encode(mkb_handle_t h, void *stream, const float *coords, int64_t frame_stride, int64_t n_frames, int64_t natoms,
+                   float precision, float scale, uint8_t *out_bytes, int64_t out_capacity, int64_t *frame_offsets,
+                   int32_t *frame_nbytes, int32_t *status);
+
 /* K10 (SURVEY 8f row 3): the kernel of the `within` / `exwithin` atom selections, replaces within_distance
  * (moleculekit/atomselect_utils/atomselect_utils.pyx:612-653; called from atomselect/atomselect.py:243-251).
  * coords [n_atoms,3] float32 device (one frame, row-major); sel1 [n1] uint32 device = query atoms (NULL = all atoms,

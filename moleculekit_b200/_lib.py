@@ -42,6 +42,7 @@ EXPORTS = [
     "mkb_dist_trajectory", "mkb_contacts_count", "mkb_contacts_fill", "mkb_dist_reduction",
     "mkb_cdist", "mkb_pdist", "mkb_squareform", "mkb_collisions_count", "mkb_collisions_fill",
     "mkb_bonds_count", "mkb_bonds_fill", "mkb_shell_counts", "mkb_wrap_box", "mkb_within_distance", "mkb_xtc_decode",
+    "mkb_xtc_encode",
     "mkb_wrap_triclinic", "mkb_hbonds_count", "mkb_hbonds_fill", "mkb_ring_pairs_count", "mkb_ring_pairs_fill",
     "mkb_align_fit", "mkb_align_apply", "mkb_rmsd", "mkb_coordinates", "mkb_coord_sums", "mkb_fluctuation",
     "mkb_frame_moments", "mkb_dihedrals", "mkb_sasa", "mkb_sasa_chunk_frames", "mkb_dssp", "mkb_dssp_chunk_frames",
@@ -58,6 +59,10 @@ class MkbError(RuntimeError):
 
 class MkbUnsupported(MkbError):
     """MKB_ERR_UNSUPPORTED: a valid request outside the domain of the entry point (callers fall back to the general one)."""
+
+
+class MkbCapacity(MkbError):
+    """MKB_ERR_CAPACITY: an output buffer is too small (the entry point says where it left the size to come back with)."""
 
 
 def load():
@@ -110,6 +115,7 @@ def load():
     lib.mkb_bonds_fill.argtypes = [vp, vp, vp, vp, vp, i64, f32, vp, vp]
     lib.mkb_within_distance.argtypes = [vp, vp, vp, i64, vp, i64, vp, i64, f32, vp]
     lib.mkb_xtc_decode.argtypes = [vp, vp, vp, i64, vp, i64, i64, vp, i64, f32, vp]
+    lib.mkb_xtc_encode.argtypes = [vp, vp, vp, i64, i64, i64, f32, f32, vp, i64, vp, vp, vp]
     lib.mkb_wrap_box.argtypes = [vp, vp, tp, vp, i64, vp, i64, C.POINTER(C.c_float)]
     lib.mkb_wrap_triclinic.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, i64, C.POINTER(C.c_float), i32]
     lib.mkb_hbonds_count.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, vp, f32, f32, i32, i32, vp, C.POINTER(i64)]
@@ -161,7 +167,7 @@ def handle(device: int = 0):
 def check(rc: int, h) -> None:
     if rc != MKB_OK:
         msg = load().mkb_last_error(h)
-        raise (MkbUnsupported if rc == -5 else MkbError)(f"libmkb200 status {rc}: {msg.decode() if msg else '?'}")
+        raise {-5: MkbUnsupported, -4: MkbCapacity}.get(rc, MkbError)(f"libmkb200 status {rc}: {msg.decode() if msg else '?'}")
 
 
 # ------------------------------------------------------------------------------------------ calls from torch tensors

@@ -17,6 +17,8 @@
 #include <cmath>
 #include <vector>
 
+#include <cub/device/device_scan.cuh>
+
 #include "common.cuh"
 
 namespace mkb {
@@ -246,6 +248,317 @@ extern "C" int mkb_xtc_decode(mkb_handle_t h, void *stream, const uint8_t *file_
     if (h->timing) MKB_CUDA(h, cudaEventRecord(h->ev[1], st));
     xtc_decode_kernel<<<(unsigned)cdiv(n_frames, 64), 64, 0, st>>>(file_bytes, file_size, d_frames, n_frames, natoms, coords,
                                                                     frame_stride, scale, status);
+    MKB_LAUNCHED(h);
+    if (h->timing) MKB_CUDA(h, cudaEventRecord(h->ev[2], st));
+    return MKB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// K21: XTC encode -- the writer's half of the codec (xdrfile_compress_coord_float, src/xdrfile.cpp; restated in
+// oracle/xtc_writer.py::compress_frame, which the tests hold this kernel to byte for byte).
+//
+// The same mapping as the decoder: ONE THREAD PER FRAME, reading element (a, d, f) of the frame-minor array, so a warp in
+// step reads 32 consecutive floats.  The length of a frame's stream is known only once it has been written, so the
+// kernel runs twice: a size pass that takes the per-frame reductions (lattice ranges, the smallest consecutive distance,
+// the overflow tests) and walks the stream counting bits, and, after an exclusive scan of the block lengths, a write pass
+// that walks it again and stores 32-bit words at the frame's offset.  Blocks are therefore packed back to back with no
+// slack, no scratch buffer and no copy.  All lattice arithmetic that the reference does in C `int` is done modulo 2^32
+// here; every float step is individually rounded (the reference binary has no FMA).
+namespace mkb {
+
+constexpr long long XTC_ENC_MAX_ATOMS = 100000000;  // 102 bits per atom at most: the byte count of a block stays an int32
+
+struct XtcEncHead {  // what the size pass found and the write pass needs
+    int minint[3], maxint[3];
+    int smallidx;
+};
+
+// MSB-first bit output in 32-bit big-endian words; without WRITE only the bit count is kept
+template <bool WRITE>
+struct XtcPut {
+    unsigned *p32;           // next word of the stream
+    unsigned long long acc;  // bits not stored yet, right-aligned
+    int n;                   // how many: < 32 between calls
+    long long nbits;         // bits sent in all
+
+    __device__ __forceinline__ void init(unsigned char *p) {
+        p32 = reinterpret_cast<unsigned *>(p);
+        acc = 0; n = 0; nbits = 0;
+    }
+    // the w <= 32 low bits of v (v has no bit above them)
+    __device__ __forceinline__ void put(int w, unsigned v) {
+        nbits += w;
+        if (WRITE) {
+            acc = (acc << w) | v;
+            n += w;
+            if (n >= 32) {
+                n -= 32;
+                *p32++ = __byte_perm((unsigned)(acc >> n), 0, 0x0123);
+            }
+        }
+    }
+    // three integers as one mixed-radix number ((a*s1 + b)*s2 + c) of nbits <= 72 bits: 8-bit chunks, least significant
+    // first, then the remaining high bits (encodeints; the inverse of XtcBits::take3).  The number is kept as a 128-bit
+    // (hi, lo) pair whatever its size: one path for every triple.
+    __device__ __forceinline__ void put3(int nbits3, unsigned a, unsigned b, unsigned c, unsigned s1, unsigned s2) {
+        if (!WRITE) { nbits += nbits3; return; }
+        const unsigned long long t = (unsigned long long)a * s1 + b;
+        unsigned long long lo = t * s2, hi = __umul64hi(t, (unsigned long long)s2);
+        lo += c;
+        hi += lo < c;
+        int left = nbits3;
+        while (left > 8) {
+            put(8, (unsigned)lo & 0xffu);
+            lo = (lo >> 8) | (hi << 56);
+            hi >>= 8;
+            left -= 8;
+        }
+        put(left, (unsigned)lo);
+    }
+    // the last partial word, its unused bits zero: this is also the XDR padding of the block
+    __device__ __forceinline__ void flush() {
+        if (WRITE && n > 0) *p32 = __byte_perm((unsigned)(acc << (32 - n)), 0, 0x0123);
+    }
+};
+
+__device__ __forceinline__ bool xtc_near(const int (&a)[3], const int (&b)[3], int lim) {  // C abs(): abs(INT_MIN) < 0
+    return abs((int)((unsigned)a[0] - (unsigned)b[0])) < lim && abs((int)((unsigned)a[1] - (unsigned)b[1])) < lim &&
+           abs((int)((unsigned)a[2] - (unsigned)b[2])) < lim;
+}
+
+template <bool WRITE>
+__global__ void __launch_bounds__(64)
+xtc_encode_kernel(const float *__restrict__ coords, long long fs, long long F, int natoms, float precision, float scale,
+                  XtcEncHead *__restrict__ heads, unsigned char *__restrict__ out, long long *__restrict__ offsets,
+                  int *__restrict__ nbytes_out, int *__restrict__ status) {
+    const long long f = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (f >= F) return;
+    const float *col = coords + f;  // element (a, d) of this frame: col[(a*3 + d) * fs]
+    const bool rescale = scale != 1.0f;
+    auto real = [&](long long w) {
+        const float x = __ldg(col + w * fs);
+        return rescale ? __fmul_rn(x, scale) : x;
+    };
+    if (natoms <= 9) {  // plain big-endian floats (xdrfile.cpp: size <= 9)
+        if (WRITE) {
+            unsigned *o = reinterpret_cast<unsigned *>(out + offsets[f]);
+            for (int w = 0; w < 3 * natoms; ++w) o[w] = __byte_perm(__float_as_uint(real(w)), 0, 0x0123);
+        } else {
+            nbytes_out[f] = 12 * natoms;
+            offsets[f + 1] = 12 * natoms;
+        }
+        return;
+    }
+    // float -> lattice: lf = x * precision, +- 0.5 by the sign of x, truncate; |lf| > INT_MAX - 2 (or not a number, where
+    // the reference's conversion is undefined) is the reference's "Internal overflow compressing coordinates"
+    bool bad = false;
+    auto lattice = [&](int a, int (&c)[3]) {
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+            const float x = real(3ll * a + d);
+            float lf = __fmul_rn(x, precision);
+            lf = x >= 0.0f ? __fadd_rn(lf, 0.5f) : __fsub_rn(lf, 0.5f);
+            bad |= !(fabs((double)lf) <= 2147483645.0);
+            c[d] = (int)lf;
+        }
+    };
+    XtcEncHead hd;
+    if (!WRITE) {
+        int mindiff = INT_MAX, old[3] = {0, 0, 0};
+#pragma unroll
+        for (int d = 0; d < 3; ++d) { hd.minint[d] = INT_MAX; hd.maxint[d] = INT_MIN; }
+        for (int a = 0; a < natoms; ++a) {
+            int c[3];
+            lattice(a, c);
+            unsigned diff = 0;
+#pragma unroll
+            for (int d = 0; d < 3; ++d) {
+                hd.minint[d] = min(hd.minint[d], c[d]);
+                hd.maxint[d] = max(hd.maxint[d], c[d]);
+                diff += (unsigned)abs((int)((unsigned)c[d] - (unsigned)old[d]));
+                old[d] = c[d];
+            }
+            if (a > 0) mindiff = min(mindiff, (int)diff);
+        }
+        int st = 0;
+        hd.smallidx = XTC_FIRSTIDX;
+        if (bad) {
+            st = MKB_XTC_ENC_COORD_OVERFLOW;
+        } else if (__fsub_rn((float)hd.maxint[0], (float)hd.minint[0]) >= 2147483648.0f ||  // (float)(INT_MAX - 2) = 2^31
+                   __fsub_rn((float)hd.maxint[1], (float)hd.minint[1]) >= 2147483648.0f ||
+                   __fsub_rn((float)hd.maxint[2], (float)hd.minint[2]) >= 2147483648.0f) {
+            st = MKB_XTC_ENC_RANGE_OVERFLOW;
+        } else {
+            while (hd.smallidx < XTC_LASTIDX && c_xtc_magic[hd.smallidx] < mindiff) ++hd.smallidx;
+            if (hd.smallidx + 8 >= XTC_LASTIDX) st = MKB_XTC_ENC_SMALLIDX_RANGE;  // the reference reads magicints[73]
+        }
+        if (st) {
+            status[f] = st;
+            nbytes_out[f] = 0;
+            offsets[f + 1] = 0;
+            return;
+        }
+        heads[f] = hd;
+    } else {
+        if (status[f] != 0) return;
+        hd = heads[f];
+    }
+    unsigned sizeint[3];
+    int bitsizeint[3] = {0, 0, 0};
+#pragma unroll
+    for (int d = 0; d < 3; ++d) sizeint[d] = (unsigned)hd.maxint[d] - (unsigned)hd.minint[d] + 1u;
+    int bitsize;
+    if ((sizeint[0] | sizeint[1] | sizeint[2]) > 0xffffffu) {
+#pragma unroll
+        for (int d = 0; d < 3; ++d) bitsizeint[d] = xtc_bits_of(sizeint[d]);
+        bitsize = 0;
+    } else {
+        bitsize = xtc_bits_of3(sizeint[0], sizeint[1], sizeint[2]);
+    }
+    int smallidx = hd.smallidx;
+    const int minidx = smallidx, maxidx = smallidx + 8;  // maxidx < LASTIDX was checked by the size pass
+    const int larger = c_xtc_magic[maxidx] / 2;
+    int smaller = c_xtc_magic[max(XTC_FIRSTIDX, smallidx - 1)] / 2;
+    int smallnum = c_xtc_magic[smallidx] / 2;
+    unsigned sizesmall = (unsigned)c_xtc_magic[smallidx];
+    unsigned char *block = WRITE ? out + offsets[f] : nullptr;
+    XtcPut<WRITE> b;
+    b.init(WRITE ? block + 36 : nullptr);
+    int prevrun = -1, prev[3] = {0, 0, 0}, nxt[3];
+    lattice(0, nxt);  // nxt = atom i in the writer's order (the first two atoms of a run trade places) while i < natoms
+    int i = 0;
+    while (i < natoms) {
+        int cur[3] = {nxt[0], nxt[1], nxt[2]};
+        int is_smaller;
+        if (smallidx < maxidx && i >= 1 && xtc_near(cur, prev, larger)) is_smaller = 1;
+        else if (smallidx > minidx) is_smaller = -1;
+        else is_smaller = 0;
+        bool is_small = false;
+        if (i + 1 < natoms) {
+            int nn[3];
+            lattice(i + 1, nn);
+            is_small = xtc_near(cur, nn, smallnum);
+#pragma unroll
+            for (int d = 0; d < 3; ++d) {
+                if (is_small) { nxt[d] = cur[d]; cur[d] = nn[d]; }  // water O then H: the second atom is sent in full
+                else nxt[d] = nn[d];
+            }
+        }
+#pragma unroll
+        for (int d = 0; d < 3; ++d) prev[d] = cur[d];
+        ++i;
+        if (!is_small && is_smaller == -1) is_smaller = 0;
+        if (bitsize == 0) {
+#pragma unroll
+            for (int d = 0; d < 3; ++d) b.put(bitsizeint[d], (unsigned)cur[d] - (unsigned)hd.minint[d]);
+        } else {
+            b.put3(bitsize, (unsigned)cur[0] - (unsigned)hd.minint[0], (unsigned)cur[1] - (unsigned)hd.minint[1],
+                   (unsigned)cur[2] - (unsigned)hd.minint[2], sizeint[1], sizeint[2]);
+        }
+        // the run: up to 8 atoms, each within smallnum of its predecessor, kept as their small offsets until the flag
+        // that precedes them in the stream is known
+        unsigned run[8][3];
+        int nrun = 0;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            if (is_small) {
+                unsigned tmpsum = 0;
+#pragma unroll
+                for (int d = 0; d < 3; ++d) {
+                    const unsigned dd = (unsigned)nxt[d] - (unsigned)prev[d];
+                    tmpsum += dd * dd;
+                    run[k][d] = dd + (unsigned)smallnum;
+                    prev[d] = nxt[d];
+                }
+                if (is_smaller == -1 && (int)tmpsum >= (int)((unsigned)smaller * (unsigned)smaller)) is_smaller = 0;
+                ++i;
+                nrun = k + 1;
+                is_small = false;
+                if (i < natoms) {
+                    lattice(i, nxt);
+                    is_small = xtc_near(nxt, prev, smallnum);
+                }
+            }
+        }
+        if (3 * nrun != prevrun || is_smaller != 0) {  // flag bit 1 and the 5-bit code
+            prevrun = 3 * nrun;
+            b.put(6, 32u | (unsigned)(3 * nrun + is_smaller + 1));
+        } else {
+            b.put(1, 0u);
+        }
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+            if (k < nrun) b.put3(smallidx, run[k][0], run[k][1], run[k][2], sizesmall, sizesmall);
+        if (is_smaller != 0) {
+            smallidx += is_smaller;
+            smaller = is_smaller < 0 ? c_xtc_magic[smallidx - 1] / 2 : smallnum;
+            smallnum = c_xtc_magic[smallidx] / 2;
+            sizesmall = (unsigned)c_xtc_magic[smallidx];
+        }
+    }
+    b.flush();
+    const int nbytes = (int)((b.nbits + 7) >> 3);
+    if (WRITE) {
+        unsigned *hw = reinterpret_cast<unsigned *>(block);
+        hw[0] = __byte_perm(__float_as_uint(precision), 0, 0x0123);
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+            hw[1 + d] = __byte_perm((unsigned)hd.minint[d], 0, 0x0123);
+            hw[4 + d] = __byte_perm((unsigned)hd.maxint[d], 0, 0x0123);
+        }
+        hw[7] = __byte_perm((unsigned)hd.smallidx, 0, 0x0123);
+        hw[8] = __byte_perm((unsigned)nbytes, 0, 0x0123);
+    } else {
+        const int len = 36 + ((nbytes + 3) & ~3);
+        nbytes_out[f] = len;
+        offsets[f + 1] = len;
+    }
+}
+
+}  // namespace mkb
+
+extern "C" int mkb_xtc_encode(mkb_handle_t h, void *stream, const float *coords, int64_t frame_stride, int64_t n_frames,
+                              int64_t natoms, float precision, float scale, uint8_t *out_bytes, int64_t out_capacity,
+                              int64_t *frame_offsets, int32_t *frame_nbytes, int32_t *status) {
+    MKB_ENTER(h);
+    cudaStream_t st = (cudaStream_t)stream;
+    MKB_STREAM_ORDER(h, st);
+    if (n_frames < 0 || natoms < 0 || out_capacity < 0) return fail(h, MKB_ERR_BAD_ARG, "negative size");
+    if (n_frames == 0 || natoms == 0) return MKB_OK;
+    if (!coords || !frame_offsets || !frame_nbytes || !status) return fail(h, MKB_ERR_BAD_ARG, "null argument");
+    if (out_capacity > 0 && !out_bytes) return fail(h, MKB_ERR_BAD_ARG, "null out_bytes with a capacity");
+    if (reinterpret_cast<uintptr_t>(out_bytes) & 3) return fail(h, MKB_ERR_BAD_ARG, "out_bytes must be 4-byte aligned");
+    if (frame_stride < n_frames) return fail(h, MKB_ERR_BAD_ARG, "frame stride < n_frames");
+    if (natoms > XTC_ENC_MAX_ATOMS) return fail(h, MKB_ERR_BAD_ARG, "too many atoms");
+    if (n_frames >= (1ll << 31) - 1) return fail(h, MKB_ERR_BAD_ARG, "too many frames for one call");
+    if (!(precision > 0.0f)) precision = 1000.0f;  // the reference's rule, before the float -> int step
+    XtcEncHead *heads;
+    int rc;
+    if ((rc = scratch_get(h, S_DESC, (size_t)n_frames, &heads))) return rc;
+    long long *offsets = reinterpret_cast<long long *>(frame_offsets);
+    size_t tmp_bytes = 0;
+    MKB_CUDA(h, cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, offsets + 1, offsets + 1, (int)n_frames, st));
+    void *tmp = nullptr;
+    if ((rc = scratch_get(h, S_SCAN_TMP, tmp_bytes, &tmp))) return rc;
+    const unsigned grid = (unsigned)cdiv(n_frames, 64);
+    if (h->timing) MKB_CUDA(h, cudaEventRecord(h->ev[0], st));
+    MKB_CUDA(h, cudaMemsetAsync(status, 0, sizeof(int32_t) * (size_t)n_frames, st));
+    MKB_CUDA(h, cudaMemsetAsync(offsets, 0, sizeof(long long), st));
+    // size pass: block lengths into frame_nbytes and, as int64, into frame_offsets[1..], which the scan turns into offsets
+    xtc_encode_kernel<false><<<grid, 64, 0, st>>>(coords, frame_stride, n_frames, (int)natoms, precision, scale, heads,
+                                                  nullptr, offsets, frame_nbytes, status);
+    MKB_LAUNCHED(h);
+    MKB_CUDA(h, cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, offsets + 1, offsets + 1, (int)n_frames, st));
+    h->launches++;
+    long long total = 0;
+    MKB_CUDA(h, cudaMemcpyAsync(&total, offsets + n_frames, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    MKB_CUDA(h, cudaStreamSynchronize(st));
+    if (total > out_capacity)
+        return fail(h, MKB_ERR_CAPACITY, "out_capacity is %lld bytes, the blocks take %lld (frame_offsets[n_frames])",
+                    (long long)out_capacity, total);
+    if (h->timing) MKB_CUDA(h, cudaEventRecord(h->ev[1], st));
+    xtc_encode_kernel<true><<<grid, 64, 0, st>>>(coords, frame_stride, n_frames, (int)natoms, precision, scale, heads,
+                                                 out_bytes, offsets, frame_nbytes, status);
     MKB_LAUNCHED(h);
     if (h->timing) MKB_CUDA(h, cudaEventRecord(h->ev[2], st));
     return MKB_OK;
