@@ -287,6 +287,38 @@ int mkb_xtc_encode(mkb_handle_t h, void *stream, const float *coords, int64_t fr
                    float precision, float scale, uint8_t *out_bytes, int64_t out_capacity, int64_t *frame_offsets,
                    int32_t *frame_nbytes, int32_t *status);
 
+/* K22: DCD (CHARMM / NAMD / OpenMM) frame records read on the device; replaces the per-frame fread and X/Y/Z -> xyz
+ * interleave of read_charmm_timestep (moleculekit/fileformats/dcd/src/dcdplugin.c) and the host transposition to the
+ * frame-minor array.  bytes = frame records on the device (4-byte aligned; every float of a DCD file sits at a multiple
+ * of 4, since all its records and markers do); frames[k] (HOST) = listed frame k: the byte offsets in `bytes` of its X, Y
+ * and Z float arrays and the floats per record.  coords (natoms, 3, n_frames) float32 device, element (a, d, k) at
+ * coords[(a*3 + d)*frame_stride + k] = float a of record d of frame k.  Values are moved as 32-bit words, never through
+ * float arithmetic: every bit pattern arrives unchanged.  swap != 0 byte-swaps every word (a file of the other byte order).
+ * Fixed atoms (header NAMNF > 0): the file's first frame holds all natoms, every later frame only the n_free free atoms.
+ * slot [natoms] int32 device = position of atom a in the free list, -1 for a fixed atom (NULL: no fixed atoms); a record
+ * of natoms floats is indexed by atom, one of n_free floats by slot[a], and a fixed atom of such a frame is read from the
+ * file's first frame, described by `first` (HOST) with offsets into first_bytes (device, first_nbytes long) -- so the first
+ * frame is the source for fixed atoms even when it is not listed.  slot values must be below n_free.  Every descriptor is
+ * checked on the host: a record outside its buffer, off a 4-byte boundary, or of another length is MKB_ERR_BAD_ARG.
+ * Bit-identical to the plugin's reader. */
+typedef struct {
+    int64_t offset[3]; /* X, Y, Z float arrays */
+    int64_t count;     /* floats per record: natoms, or n_free for a later frame of a file with fixed atoms */
+} mkb_dcd_frame;
+int mkb_dcd_decode(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t nbytes, const mkb_dcd_frame *frames,
+                   int64_t n_frames, int64_t natoms, const int32_t *slot, int64_t n_free, const uint8_t *first_bytes,
+                   int64_t first_nbytes, const mkb_dcd_frame *first, int32_t swap, float *coords, int64_t frame_stride);
+
+/* K22: DCD frame records written on the device, the inverse of mkb_dcd_decode; replaces the frame loop of the plugin's
+ * write_dcdstep.  coords float32 device, element (a, d, k) at coords[(a*3 + d)*frame_stride + k]; unitcell [n_frames][6]
+ * float64 device (A, cos gamma, B, cos beta, cos alpha, C) or NULL.  Frame k is written at out + k*S, S = 56 (with a unit
+ * cell) + 3*(8 + 4*natoms) bytes: the unit-cell record [48, 6 doubles, 48] when unitcell != NULL, then the X, Y and Z
+ * records [4*natoms, natoms floats, 4*natoms], all little-endian (the plugin's native order on x86), no fixed atoms.  out
+ * is 4-byte aligned, unitcell 8-byte aligned; n_frames*S > out_capacity is MKB_ERR_CAPACITY and 4*natoms beyond the
+ * int32 record markers MKB_ERR_BAD_ARG.  Byte-identical to the plugin's frame records. */
+int mkb_dcd_encode(mkb_handle_t h, void *stream, const float *coords, int64_t frame_stride, int64_t n_frames, int64_t natoms,
+                   const double *unitcell, uint8_t *out, int64_t out_capacity);
+
 /* K10 (SURVEY 8f row 3): the kernel of the `within` / `exwithin` atom selections, replaces within_distance
  * (moleculekit/atomselect_utils/atomselect_utils.pyx:612-653; called from atomselect/atomselect.py:243-251).
  * coords [n_atoms,3] float32 device (one frame, row-major); sel1 [n1] uint32 device = query atoms (NULL = all atoms,
