@@ -319,6 +319,26 @@ int mkb_dcd_decode(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t n
 int mkb_dcd_encode(mkb_handle_t h, void *stream, const float *coords, int64_t frame_stride, int64_t n_frames, int64_t natoms,
                    const double *unitcell, uint8_t *out, int64_t out_capacity);
 
+/* K23: AMBER NetCDF (netCDF-3) trajectory coordinates read on the device; replaces the host read of the big-endian
+ * `coordinates` variable (frame, atom, spatial) (moleculekit/fileformats/netcdf.py) and the host transposition to the
+ * frame-minor array.  bytes = staged file bytes on the device (4-byte aligned); offsets[k] (HOST) = byte offset in
+ * `bytes` of listed frame k's 12*natoms coordinate bytes (big-endian float32, atom-major, x y z per atom), >= 0, a
+ * multiple of 4 and with offsets[k] + 12*natoms <= nbytes, else MKB_ERR_BAD_ARG.  coords (natoms, 3, n_frames) float32
+ * device, element (a, d, k) at coords[(a*3 + d)*frame_stride + k].  Values are byte-swapped as 32-bit words, never
+ * passed through float arithmetic: every bit pattern arrives unchanged. */
+int mkb_netcdf_decode(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t nbytes, const int64_t *offsets,
+                      int64_t n_frames, int64_t natoms, float *coords, int64_t frame_stride);
+
+/* K23: AMBER NetCDF records written on the device, the inverse of mkb_netcdf_decode.  coords float32 device, element
+ * (a, d, k) at coords[(a*3 + d)*frame_stride + k].  Record k is written at out + k*record_bytes: its coordinates
+ * big-endian at coord_offset, and the other record_bytes - 12*natoms bytes from extra + k*(record_bytes - 12*natoms)
+ * (device, already in file byte order; NULL when there are none): the first coord_offset of them before the
+ * coordinates, the rest after.  record_bytes and coord_offset are multiples of 4 with coord_offset + 12*natoms <=
+ * record_bytes; out, extra and coords are 4-byte aligned.  n_frames*record_bytes > out_capacity is MKB_ERR_CAPACITY. */
+int mkb_netcdf_encode(mkb_handle_t h, void *stream, const float *coords, int64_t frame_stride, int64_t n_frames,
+                      int64_t natoms, int64_t record_bytes, int64_t coord_offset, const uint8_t *extra, uint8_t *out,
+                      int64_t out_capacity);
+
 /* K10 (SURVEY 8f row 3): the kernel of the `within` / `exwithin` atom selections, replaces within_distance
  * (moleculekit/atomselect_utils/atomselect_utils.pyx:612-653; called from atomselect/atomselect.py:243-251).
  * coords [n_atoms,3] float32 device (one frame, row-major); sel1 [n1] uint32 device = query atoms (NULL = all atoms,

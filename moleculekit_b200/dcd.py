@@ -37,7 +37,7 @@ import struct
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, _trajio
 
 logger = logging.getLogger(__name__)
 
@@ -308,23 +308,6 @@ def decode_dcd_device(buf: torch.Tensor, frames: np.ndarray, natoms: int, swap: 
     return out
 
 
-def _chunks(sel: np.ndarray, size: np.ndarray, chunk_bytes: int) -> list:
-    """Cut the listed frames, in order, into chunks whose distinct frames take at most ``chunk_bytes`` (one frame at
-    least): [(k0, k1, sorted distinct frames)]."""
-    out, k0, seen, used = [], 0, set(), 0
-    for k, j in enumerate(sel.tolist()):
-        if j in seen:
-            continue
-        if seen and used + size[j] > chunk_bytes:
-            out.append((k0, k, np.array(sorted(seen), np.int64)))
-            k0, seen, used = k, set(), 0
-        seen.add(j)
-        used += int(size[j])
-    if len(sel):
-        out.append((k0, len(sel), np.array(sorted(seen), np.int64)))
-    return out
-
-
 def read_dcd_device(filename, frames=None, device=None, chunk_bytes: int = CHUNK_BYTES):
     """Whole file (or the frames listed: any order, repeats allowed) -> (coords CUDA (natoms, 3, F) float32 [Angstrom],
     box (3, F) float32, boxangles (3, F) float32, info dict) with the trajectory left on the GPU.  ``info`` holds istart,
@@ -347,7 +330,7 @@ def read_dcd_device(filename, frames=None, device=None, chunk_bytes: int = CHUNK
     if n == 0 or natoms == 0:
         return coords, idx["box"][:, sel], idx["boxangles"][:, sel], info
     start, size, fdesc = idx["start"], idx["size"], idx["frames"]
-    chunks = _chunks(sel, size, int(chunk_bytes))
+    chunks = _trajio.chunks(sel, size, int(chunk_bytes))
     cap = max(int(size[u].sum()) for _, _, u in chunks)
     stream = torch.cuda.current_stream(dev)
     with open(filename, "rb") as fh:
@@ -418,15 +401,6 @@ def dcd_header(natoms: int, n_frames: int, istart: int = 0, nsavc: int = 1, delt
     return cord + struct.pack("<ii", n, len(lines)) + text + struct.pack("<iiii", n, 4, natoms, 4)
 
 
-def _frame_minor(coords: torch.Tensor) -> torch.Tensor:
-    """``coords`` as it is when it is (natoms, 3, F) frame-minor (a frame slice included), else a contiguous copy"""
-    N, _, F = coords.shape
-    s_atom, s_axis, s_frame = coords.stride()
-    if N and F and not (s_atom == 3 * s_axis and (F == 1 or s_frame == 1) and s_axis >= F):
-        coords = coords.contiguous()
-    return coords
-
-
 def _writer_args(coords, box, boxangles, istart, nsavc, title):
     """shapes and ranges checked before any device work; returns (natoms, F)"""
     if coords.ndim != 3 or coords.shape[1] != 3:
@@ -473,7 +447,7 @@ def _encode(coords, cells, natoms: int, F: int, out: torch.Tensor | None = None)
         out = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     if F == 0:
         return out[:0]
-    coords = _frame_minor(coords)
+    coords = _trajio.frame_minor(coords)
     stride = coords.stride(1) if natoms else F
     _lib.call(dev, "mkb_dcd_encode", _lib.ptr(coords) if natoms else None, max(int(stride), F), F, natoms,
               _lib.ptr(cells), _lib.ptr(out), int(out.numel()))
@@ -500,30 +474,9 @@ def _write(fh, coords, box, boxangles, istart, nsavc, delta, title, device, chun
         dev = _lib.device(device)
         coords = torch.from_numpy(np.ascontiguousarray(coords)).to(dev)
     cells = None if box is None else torch.from_numpy(box_to_unitcell(box, boxangles)).to(dev)
-    S = _frame_bytes(natoms, cells is not None)
-    per = max(1, min(F, int(chunk_bytes) // S))
-    spans = [(f0, min(F, f0 + per)) for f0 in range(0, F, per)]
-    n_buf = min(2, len(spans))
-    devb = [torch.empty(per * S, dtype=torch.uint8, device=dev) for _ in range(n_buf)]
-    host = [torch.empty(per * S, dtype=torch.uint8, pin_memory=True) for _ in range(n_buf)]
-    done = [None] * n_buf
-    stream = torch.cuda.current_stream(dev)
-    pending = None  # (buffer, bytes) copied to the host but not yet written
-    for c, (f0, f1) in enumerate(spans):
-        i = c % n_buf
-        _encode(coords[:, :, f0:f1], None if cells is None else cells[f0:f1], natoms, f1 - f0, out=devb[i])
-        nbytes = (f1 - f0) * S
-        host[i][:nbytes].copy_(devb[i][:nbytes], non_blocking=True)
-        done[i] = torch.cuda.Event()
-        done[i].record(stream)
-        if pending is not None:  # write the previous chunk while this one encodes and copies
-            j, nb = pending
-            done[j].synchronize()
-            fh.write(memoryview(host[j].numpy())[:nb])
-        pending = (i, nbytes)
-    j, nb = pending
-    done[j].synchronize()
-    fh.write(memoryview(host[j].numpy())[:nb])
+    _trajio.write_encoded(fh, dev, F, _frame_bytes(natoms, cells is not None), chunk_bytes,
+                          lambda f0, f1, out: _encode(coords[:, :, f0:f1], None if cells is None else cells[f0:f1],
+                                                      natoms, f1 - f0, out=out))
 
 
 def dcd_bytes(coords, box=None, boxangles=None, istart: int = 0, nsavc: int = 1, delta: float = 1.0, title=None,
