@@ -339,6 +339,34 @@ int mkb_netcdf_encode(mkb_handle_t h, void *stream, const float *coords, int64_t
                       int64_t natoms, int64_t record_bytes, int64_t coord_offset, const uint8_t *extra, uint8_t *out,
                       int64_t out_capacity);
 
+/* K24: GROMACS TRR x, v or f blocks read on the device; replaces xdrfile's read_trr (moleculekit/fileformats/xtc/trr.pyx
+ * over xdrfile_trr.c), which returns each frame's block as (natoms, 3) reals, and the host transposition to the
+ * frame-minor array.  bytes = staged file bytes on the device; offsets[k] (HOST) = byte offset in `bytes` of listed frame
+ * k's block: 3*natoms big-endian XDR reals of value_bytes (4: float32, 8: float64) each, atom-major, x y z per atom.
+ * value_bytes is 4 or 8; bytes and every offset are multiples of value_bytes, offsets[k] >= 0 and offsets[k] +
+ * 3*natoms*value_bytes <= nbytes, else MKB_ERR_BAD_ARG.  A float64 block in a file starts on a 4-byte boundary only (the
+ * double-precision header is 92 bytes), so 8-byte reals are read with 64-bit loads from a staging buffer the caller
+ * lays out at multiples of 8 (moleculekit_b200.trr stages every block in its own row of 24*natoms bytes), not from the
+ * file's own offsets.  coords (natoms, 3, n_frames) float32 device, element (a, d, k) at coords[(a*3 + d)*frame_stride +
+ * k].  4-byte reals are byte-swapped as 32-bit words, never passed through float arithmetic: every bit pattern arrives
+ * unchanged.  8-byte reals are rounded to float32 exactly as x86-64's cvtsd2ss (numpy's astype(np.float32)) does:
+ * to nearest, ties to even, overflow to +-inf, float32 subnormals kept; a NaN gives sign | 0x7fc00000 | (its 52-bit
+ * mantissa >> 29). */
+int mkb_trr_decode(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t nbytes, const int64_t *offsets,
+                   int64_t n_frames, int64_t natoms, int32_t value_bytes, float *coords, int64_t frame_stride);
+
+/* K24: single-precision GROMACS TRR frames written on the device, the inverse of mkb_trr_decode for 4-byte reals;
+ * replaces the frame loop of xdrfile's write_trr.  x, v, f float32 device (v and f NULL when absent), each element
+ * (a, d, k) at p[(a*3 + d)*frame_stride + k]: one frame stride for all three.  Frame k is written at out + k*R, R =
+ * head_bytes + (1 + (v != NULL) + (f != NULL))*12*natoms: its head_bytes bytes from head + k*head_bytes (device, already
+ * in file byte order -- the writer puts the 84-byte frame header and the 36-byte box there), then x, then v and f when
+ * given, each as 3*natoms big-endian float32.  head_bytes is a multiple of 4; x, v, f, head and out are 4-byte aligned.
+ * n_frames*R > out_capacity is MKB_ERR_CAPACITY.  Values are byte-swapped as 32-bit words: every bit pattern is
+ * written unchanged. */
+int mkb_trr_encode(mkb_handle_t h, void *stream, const float *x, const float *v, const float *f, int64_t frame_stride,
+                   int64_t n_frames, int64_t natoms, const uint8_t *head, int64_t head_bytes, uint8_t *out,
+                   int64_t out_capacity);
+
 /* K10 (SURVEY 8f row 3): the kernel of the `within` / `exwithin` atom selections, replaces within_distance
  * (moleculekit/atomselect_utils/atomselect_utils.pyx:612-653; called from atomselect/atomselect.py:243-251).
  * coords [n_atoms,3] float32 device (one frame, row-major); sel1 [n1] uint32 device = query atoms (NULL = all atoms,

@@ -1,9 +1,15 @@
-"""Host plumbing shared by the trajectory file modules that transpose frame records on the device (``dcd``, ``netcdf``):
-the chunk planner of a frame list, the frame-minor layout check, and the double-buffered encode -> copy -> write loop."""
+"""Host plumbing shared by the trajectory file modules that transpose frame records on the device (``dcd``, ``netcdf``,
+``trr``): the chunk planner of a frame list, the slab gather into staging rows, the frame-minor layout check, and the
+double-buffered encode -> copy -> write loop."""
 from __future__ import annotations
+
+import os
 
 import numpy as np
 import torch
+
+IOV_MAX = 1024  # buffers per preadv call (Linux)
+PREADV_BYTES = 1 << 30  # slab bytes per preadv call, well below the 2 GiB a single read returns at most
 
 
 def chunks(sel: np.ndarray, size: np.ndarray, chunk_bytes: int) -> list:
@@ -21,6 +27,29 @@ def chunks(sel: np.ndarray, size: np.ndarray, chunk_bytes: int) -> list:
     if len(sel):
         out.append((k0, len(sel), np.array(sorted(seen), np.int64)))
     return out
+
+
+def gather_slabs(fd: int, starts: np.ndarray, slab: int, out: np.ndarray, fmt: str) -> None:
+    """Read the ``slab`` bytes at each file offset of ``starts`` (ascending) into the rows of ``out`` (len(starts), slab).
+    A run of slabs whose gaps are small is one ``preadv``: the slabs land in their rows, the bytes between them (the
+    record's other variables) in a scratch buffer, so the page cache is copied once and no gap reaches ``out``.  A short
+    read raises RuntimeError("Malformed ``fmt`` file: ...")."""
+    junk = memoryview(bytearray(max(slab, 1 << 20)))
+    n, k = len(starts), 0
+    while k < n:
+        iov, j = [memoryview(out[k])], k
+        while j + 1 < n and len(iov) + 2 <= IOV_MAX and (j + 2 - k) * slab <= PREADV_BYTES:
+            gap = int(starts[j + 1] - starts[j]) - slab
+            if not 0 <= gap <= len(junk):
+                break
+            if gap:
+                iov.append(junk[:gap])
+            iov.append(memoryview(out[j + 1]))
+            j += 1
+        want = sum(len(v) for v in iov)
+        if os.preadv(fd, iov, int(starts[k])) != want:
+            raise RuntimeError(f"Malformed {fmt} file: the file changed while it was read")
+        k = j + 1
 
 
 def frame_minor(coords: torch.Tensor) -> torch.Tensor:

@@ -53,8 +53,6 @@ MAX_ATOMS = (2**31 - 1) // 12  # a coordinate slab of 12 * natoms bytes must fit
 MAX_FRAMES = 2**31 - 1  # numrecs is a non-negative int32 in a classic file
 DEFAULT_TITLE = "written by moleculekit_b200"
 CHUNK_BYTES = 256 << 20
-IOV_MAX = 1024  # buffers per preadv call (Linux)
-PREADV_BYTES = 1 << 30  # slab bytes per preadv call, well below the 2 GiB a single read returns at most
 # the host-built part of a record, in file byte order: time, then (with a box) cell_lengths and cell_angles
 EXTRA_BOX = np.dtype([("time", ">f4"), ("lengths", ">f8", (3,)), ("angles", ">f8", (3,))], align=False)
 EXTRA_NOBOX = np.dtype([("time", ">f4")])
@@ -282,25 +280,8 @@ def decode_netcdf_device(buf: torch.Tensor, offsets, natoms: int, out: torch.Ten
 
 
 def _gather_slabs(fd: int, starts: np.ndarray, slab: int, out: np.ndarray) -> None:
-    """Read the ``slab`` bytes at each file offset of ``starts`` (ascending) into the rows of ``out`` (len(starts), slab).
-    A run of slabs whose gaps are small is one ``preadv``: the slabs land in their rows, the bytes between them (the
-    record's other variables) in a scratch buffer, so the page cache is copied once and no gap reaches ``out``."""
-    junk = memoryview(bytearray(max(slab, 1 << 20)))
-    n, k = len(starts), 0
-    while k < n:
-        iov, j = [memoryview(out[k])], k
-        while j + 1 < n and len(iov) + 2 <= IOV_MAX and (j + 2 - k) * slab <= PREADV_BYTES:
-            gap = int(starts[j + 1] - starts[j]) - slab
-            if not 0 <= gap <= len(junk):
-                break
-            if gap:
-                iov.append(junk[:gap])
-            iov.append(memoryview(out[j + 1]))
-            j += 1
-        want = sum(len(v) for v in iov)
-        if os.preadv(fd, iov, int(starts[k])) != want:
-            raise _malformed("the file changed while it was read")
-        k = j + 1
+    """:func:`_trajio.gather_slabs` for a NetCDF file"""
+    _trajio.gather_slabs(fd, starts, slab, out, "NetCDF")
 
 
 def read_netcdf_device(filename, frames=None, device=None, chunk_bytes: int = CHUNK_BYTES):
