@@ -367,6 +367,34 @@ int mkb_trr_encode(mkb_handle_t h, void *stream, const float *x, const float *v,
                    int64_t n_frames, int64_t natoms, const uint8_t *head, int64_t head_bytes, uint8_t *out,
                    int64_t out_capacity);
 
+/* K25: AMBER ASCII trajectory (mdcrd / mdvel) frames parsed on the device; replaces a host reader that converts every
+ * 8-character field with float() and the host transposition to the frame-minor array.  A frame holds 3*natoms F8.3
+ * fields atom-major (x y z per atom), ten to a line: value j at byte 8*j + j/10, a newline after every value with
+ * j % 10 == 9 and after the last; with with_box != 0 one more line of three F8.3 fields (A, B, C) and a newline.  Frame
+ * bytes S = 24*natoms + ceil(3*natoms/10) + (with_box ? 25 : 0).  A field is spaces, an optional '-', digits, '.' and
+ * three digits.  bytes = staged file bytes on the device, 16-byte aligned; offsets[k] (HOST) = byte offset in `bytes`
+ * of listed frame k, >= 0, a multiple of 16, with offsets[k] + S rounded up to 4 <= nbytes (the kernel reads whole
+ * aligned words), else MKB_ERR_BAD_ARG.  coords (natoms, 3, n_frames) float32 device, element (a, d, k) at
+ * coords[(a*3 + d)*frame_stride + k]; box (3, n_frames) float32 device at box[d*box_stride + k], used only with a box.
+ * A field's digits k (point removed) give __double2float_rn(k / 1000.0) with its sign, bit for bit
+ * np.float32(float(field)) ('-0.000' is -0.0).  bad (device int64, 8-byte aligned, set to INT64_MAX by the caller)
+ * receives the atomic minimum of k*S + b over the malformed bytes b of listed frame k: a field that breaks the grammar
+ * (b = its first byte) or a byte that is not the newline the layout puts there.  The values decoded from a malformed
+ * frame are unspecified. */
+int mkb_mdcrd_decode(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t nbytes, const int64_t *offsets,
+                     int64_t n_frames, int64_t natoms, int32_t with_box, float *coords, int64_t frame_stride,
+                     float *box, int64_t box_stride, int64_t *bad);
+
+/* K25: AMBER ASCII trajectory frames written on the device, the inverse of mkb_mdcrd_decode.  coords float32 device,
+ * element (a, d, k) at coords[(a*3 + d)*frame_stride + k]; box (3, n_frames) float32 device at box[d*box_stride + k], or
+ * NULL for frames without a box line.  Frame k is written at out + k*S (S as for mkb_mdcrd_decode, with_box = box !=
+ * NULL), byte for byte Python's '%8.3f' % x: k = rint(x * 1000) in float64 (exact, half to even), the sign printed
+ * whenever x is negative or -0.0.  A value outside the writable range (rint(x * 1000) > 9 999 999 for x >= 0, < -999 999
+ * for x < 0) or not finite is written as '********'.  The title line is the caller's.  coords, box and out are 4-byte
+ * aligned; n_frames*S > out_capacity is MKB_ERR_CAPACITY. */
+int mkb_mdcrd_encode(mkb_handle_t h, void *stream, const float *coords, int64_t frame_stride, int64_t n_frames,
+                     int64_t natoms, const float *box, int64_t box_stride, uint8_t *out, int64_t out_capacity);
+
 /* K10 (SURVEY 8f row 3): the kernel of the `within` / `exwithin` atom selections, replaces within_distance
  * (moleculekit/atomselect_utils/atomselect_utils.pyx:612-653; called from atomselect/atomselect.py:243-251).
  * coords [n_atoms,3] float32 device (one frame, row-major); sel1 [n1] uint32 device = query atoms (NULL = all atoms,
