@@ -395,6 +395,47 @@ int mkb_mdcrd_decode(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t
 int mkb_mdcrd_encode(mkb_handle_t h, void *stream, const float *coords, int64_t frame_stride, int64_t n_frames,
                      int64_t natoms, const float *box, int64_t box_stride, uint8_t *out, int64_t out_capacity);
 
+/* K26: the index pass over a chunk of a multi-frame XYZ file; replaces the host reader's line loop (readline, split()
+ * and int() per frame) as far as finding the frames.  A frame is P = natoms + 2 lines: the atom count, a comment and
+ * natoms atom lines.  bytes = the chunk on the device, 16-byte aligned: the file's bytes [file_base, file_base + n_read),
+ * of which the newlines in the first n are counted (n_read - n bytes of look-ahead, up to 64, let the last lines of the
+ * chunk be checked).  state (device int64[3], 8-byte aligned; the caller sets {0, INT64_MAX, 0} before the first chunk
+ * and keeps it across chunks, which run in file order on one stream): [0] the running newline count, [1] the atomic
+ * minimum file offset of a CR not followed by LF, [2] one more than the largest frame number past frame_cap.  Every line
+ * L (0-based in the file) with L % P == 0 and L >= P that starts inside the look-ahead window gets frame_off[L / P] =
+ * its file offset and status[L / P] = 0 when its first field is natoms written as [+]digits (ASCII separators before
+ * it, a separator after it, within 64 bytes), 1 when the host must decide (frame_off, status device, frame_cap
+ * entries).  Frame 0 is the caller's. */
+int mkb_xyz_index(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t n, int64_t n_read, int64_t file_base,
+                  int64_t natoms, int64_t *state, int64_t *frame_off, uint8_t *status, int64_t frame_cap);
+
+/* K26: XYZ frames parsed on the device; replaces the host reader's split() and float() per atom line and the host
+ * transposition to the frame-minor array.  bytes = n_staged whole frames back to back on the device, 16-byte aligned,
+ * nbytes long and readable up to nbytes rounded up to 16; each frame's P = natoms + 2 lines end in '\n' (the last
+ * frame's last line may end at nbytes instead).  frame_of (HOST int32[n_frames]) = the staged frame of listed frame k.
+ * coords (natoms, 3, n_frames) float32 device, element (a, d, k) at coords[(a*3 + d)*frame_stride + k] = field d + 1 of
+ * atom line a, bit for bit np.float32(float(field)): the correctly rounded double rounded to float32 (field 0 and
+ * fields past 3 are skipped).  Separators are the bytes str.split() splits ASCII text on (\t \n \v \f \r, space,
+ * 0x1c-0x1f).  A line with fewer than four fields, a byte >= 0x80 up to its fourth field, a field outside
+ * [+-]?(d+.?d*|.d+)([eE][+-]?d+)? and nan / inf / infinity, or a conversion the device cannot decide is flagged: flags
+ * (device int64, 8-byte aligned, flags[0] set to 0 by the caller) receives at flags[1 + 2 j], flags[2 + 2 j] the pair
+ * ((frame_base + k) * natoms + a, byte offset of the line from its frame's first byte) for j < flag_cap, and flags[0]
+ * counts every flagged line; such a line's coordinates are unspecified. */
+int mkb_xyz_decode(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t nbytes, int64_t n_staged,
+                   const int32_t *frame_of, int64_t n_frames, int64_t natoms, float *coords, int64_t frame_stride,
+                   int64_t frame_base, int64_t *flags, int64_t flag_cap);
+
+/* K26: XYZ frames written on the device, the inverse of mkb_xyz_decode.  coords float32 device, element (a, d, k) at
+ * coords[(a*3 + d)*frame_stride + k].  Frame k is written at out + k*S, S = head_bytes + natoms*(width + 49): the
+ * head_bytes bytes of head (device: the count and comment lines), then per atom its element column elements[a*width
+ * ...] (device, width bytes, 1 <= width <= 256) and ' %15.8f' of x, y and z, and '\n': byte for byte Python's
+ * '%-*s %15.8f %15.8f %15.8f\n'.  k = rint(x * 1e8) in float64 (exact, half to even); the caller keeps |k| below 10^14
+ * (10^13 for a negative sign) and NaN / inf out.  coords and out are 4-byte aligned; n_frames*S > out_capacity is
+ * MKB_ERR_CAPACITY. */
+int mkb_xyz_encode(mkb_handle_t h, void *stream, const float *coords, int64_t frame_stride, int64_t n_frames,
+                   int64_t natoms, const uint8_t *head, int64_t head_bytes, const uint8_t *elements, int64_t width,
+                   uint8_t *out, int64_t out_capacity);
+
 /* K10 (SURVEY 8f row 3): the kernel of the `within` / `exwithin` atom selections, replaces within_distance
  * (moleculekit/atomselect_utils/atomselect_utils.pyx:612-653; called from atomselect/atomselect.py:243-251).
  * coords [n_atoms,3] float32 device (one frame, row-major); sel1 [n1] uint32 device = query atoms (NULL = all atoms,

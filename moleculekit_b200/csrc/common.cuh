@@ -48,6 +48,10 @@ enum ScratchSlot {
     S_TMSCORE_MASK, // K19: two cut-set bitmasks per resident thread
     S_MOMENT_TAB,   // K20: segment table, group offsets / totals and weights, uploaded per call
     S_MOMENT_PART,  // K20: per-(segment, frame) partial moment sums
+    S_XYZ_COUNTS,   // K26: newlines per 32 KB segment
+    S_XYZ_BASE,     // K26: number of the first newline of every segment
+    S_XYZ_STARTS,   // K26: line starts of the staged frames
+    S_XYZ_STATE,    // K26: the decode's running line count
     S_NSLOTS
 };
 
