@@ -9,8 +9,10 @@
 //            its 8 warps split the segment's atoms and combine in shared memory, the solve kernel adds the segments in
 //            order.  The segment count depends only on the selection size, so a frame's summation order depends only on
 //            the selection: a frame slice gives the same bits as the whole call.  One reference frame: the reference is
-//            centred once (align_ref_center_kernel) and H = sum (p - p_s) q'^T; matching frames: sums relative to the first
-//            selected atom of each frame and H = S_pq - S_p S_q^T / k.  The solve kernel (one thread per frame) takes the
+//            centred once (align_ref_center_kernel) and H = sum (p - p_s) q'^T - S_p (sum q')^T / k, the second term
+//            removing what the rounding of the float64 centroid leaves in sum q' (far from the origin it would otherwise
+//            tilt H by k (p_bar - p_s) times that error); matching frames: sums relative to the first selected atom of
+//            each frame and H = S_pq - S_p S_q^T / k.  The solve kernel (one thread per frame) takes the
 //            eigenvector of the largest eigenvalue of Horn's symmetric 4x4 matrix by cyclic Jacobi in float64: det R = +1
 //            by construction, ties go to the lowest index (H = 0 gives the identity, as numpy's SVD of a zero matrix).
 //   apply    align_apply_kernel: x' = fl32(R (x - p) + q) in float64, one thread per (frame, atom stride), the frame's
@@ -47,7 +49,7 @@ struct AlignArgs {
     long long k;
     const unsigned *frames;
     long long n;      // listed frames
-    const double *qc; // FIT_SINGLE: centred reference [k][3]
+    const double *qc; // FIT_SINGLE: centred reference [k][3], q_bar [3], sum q' [3]
     const double *rec;  // RMSD: per-frame fit records, NULL = no transform
     int nseg;
     long long seg_len;
@@ -162,7 +164,7 @@ __global__ void __launch_bounds__(AL_THREADS) align_partial_kernel(const AlignAr
 }
 
 // centroid of the reference selection (fixed-order tree over one CTA) and the centred reference q' = q - q_bar;
-// qc[3k .. 3k+2] = q_bar
+// qc[3k .. 3k+2] = q_bar, qc[3k+3 .. 3k+5] = sum q' (the same tree): not zero, as q_bar is rounded
 __global__ void __launch_bounds__(AL_THREADS) align_ref_center_kernel(const float *__restrict__ ref, long long rfs,
                                                                       const unsigned *__restrict__ refsel, long long k,
                                                                       double *__restrict__ qc) {
@@ -185,12 +187,31 @@ __global__ void __launch_bounds__(AL_THREADS) align_ref_center_kernel(const floa
         __syncthreads();
     }
     const double qb[3] = {s[0][0] / (double)k, s[1][0] / (double)k, s[2][0] / (double)k};
+    __syncthreads();  // every thread has read s[.][0]
+    double r[3] = {0.0, 0.0, 0.0};
     for (long long i = t; i < k; i += AL_THREADS) {
         const float *q = ref + (long long)refsel[i] * 3 * rfs;
 #pragma unroll
-        for (int d = 0; d < 3; ++d) qc[i * 3 + d] = (double)q[d * rfs] - qb[d];
+        for (int d = 0; d < 3; ++d) {
+            const double c = (double)q[d * rfs] - qb[d];
+            qc[i * 3 + d] = c;
+            r[d] += c;
+        }
     }
-    if (t < 3) qc[3 * k + t] = s[t][0] / (double)k;
+#pragma unroll
+    for (int d = 0; d < 3; ++d) s[d][t] = r[d];
+    __syncthreads();
+    for (int h = AL_THREADS / 2; h > 0; h >>= 1) {
+        if (t < h) {
+#pragma unroll
+            for (int d = 0; d < 3; ++d) s[d][t] += s[d][t + h];
+        }
+        __syncthreads();
+    }
+    if (t < 3) {
+        qc[3 * k + t] = qb[t];
+        qc[3 * k + 3 + t] = s[t][0];
+    }
 }
 
 // one Jacobi rotation of the symmetric 4x4 `a` zeroing a[P][Q]; eigenvectors accumulate in the columns of v
@@ -303,7 +324,9 @@ __global__ void align_solve_kernel(const AlignArgs A, const double *__restrict__
 #pragma unroll
         for (int d = 0; d < 3; ++d) qb[d] = A.qc[3 * A.k + d];
 #pragma unroll
-        for (int j = 0; j < 9; ++j) H[j] = acc[3 + j];
+        for (int r = 0; r < 3; ++r)
+#pragma unroll
+            for (int c = 0; c < 3; ++c) H[3 * r + c] = acc[3 + 3 * r + c] - acc[r] * A.qc[3 * A.k + 3 + c] / k;
     }
     bool finite = true;
 #pragma unroll
@@ -413,7 +436,7 @@ extern "C" int mkb_align_fit(mkb_handle_t h, void *stream, const mkb_traj *t, co
     if ((rc = scratch_get(h, S_ALIGN_PART, (size_t)(A.nseg * nacc * A.n), &partial))) return rc;
     if (h->timing) MKB_CUDA(h, cudaEventRecord(h->ev[0], st));
     if (!A.ref_match) {
-        if ((rc = scratch_get(h, S_ALIGN_REF, (size_t)(3 * n_sel + 3), &qc))) return rc;
+        if ((rc = scratch_get(h, S_ALIGN_REF, (size_t)(3 * n_sel + 6), &qc))) return rc;
         align_ref_center_kernel<<<1, AL_THREADS, 0, st>>>(ref->coords, ref->frame_stride, refsel, n_sel, qc);
         MKB_LAUNCHED(h);
         A.qc = qc;
