@@ -196,19 +196,38 @@ __device__ __forceinline__ float pair_d2_fastwrap_flag(const float4 a, const flo
 }
 
 // Contact maps only need the BOOLEAN d2 <= T of the reference's float32 sequence, not its bits.  A fused estimate of d2
-// (3 instead of 8 instructions per axis) decides every pair whose estimate lies outside a 4e-6 band around T; pairs inside
-// the band, pairs with NaN / out-of-range quotients, and whole frames whose box is too small for the shortcut take the exact
-// sequence.  Why this is the reference's answer: (a) when the estimate's image integer n equals the reference's
-// roundf(fl(d/b)), the two d2 differ by < 1e-6 relative (a handful of float roundings); (b) when the integers differ, d/b
-// is within 1e-6 of a half-integer, so |w| >= b/2 (1 - 1e-5) in BOTH computations and both d2 exceed T as long as
-// (b/2)^2 (1 - 1e-4) > T -- checked once per frame (`shortcut`), else the exact sequence is used throughout.
-__device__ __forceinline__ bool contact_shortcut_ok(const BoxF &bx, float T) {
+// (3 instead of 8 instructions per axis) decides every pair less than QMAX = 8 boxes apart (qm = max |d/b| < 8) whose
+// estimate lies outside the band  B = 4e-6 T + 2.5e-7 thr bmax (QMAX + 1/2)  around T; pairs inside the band, farther
+// pairs, NaN quotients, and whole frames whose box is too small for the shortcut take the exact sequence.  Why this is
+// the reference's answer (u = 2^-24):
+// (a) When the estimate's image integer n equals the reference's roundf(fl(d/b)), the estimate's w = fl(d - b n) is off
+//     the exact d - b n by u |w|, while the reference's fl(d - fl(b n)) is off by up to u |b n| + u |w|: the rounding of
+//     fl(b n) grows with the distance between the images, not with |w| (at thr = 3 A it alone moves d2 by more than 4e-6
+//     relative from |d| ~ 130 A on, so the band has to grow with bmax and the quotient limit).  Summed over the axes,
+//     |d2_est - d2_ref| <= 10 u d2 + 2u |w| |b n|, and with |b n| <= sqrt(3) bmax (QMAX + 1/2) and d2 <= 1.25 T inside
+//     the band that is below B -- as long as B <= T / 4, checked once per frame.
+// (b) When the integers differ, d/b is within 2u |d/b| of a half-integer; for qm < 8 that puts |w| >= b/2 (1 - 3e-6) in
+//     BOTH computations (the reference's fl(b n) included), so both d2 exceed T as long as (b/2)^2 (1 - 1e-4) > T --
+//     checked once per frame; the estimate then answers "no contact" like the reference, or lands in the band.
+// The band is one number per frame, so the per-pair test costs what a fixed band costs.  tests/test_contact_shortcut_cpu.py
+// restates both float32 sequences and checks the rule from 0 to 2^21 boxes apart.
+struct ContactBand {
+    float band;  // B
+    bool ok;     // the shortcut's argument holds for this frame's box and threshold
+};
+constexpr float CONTACT_QMAX = 8.0f;
+__device__ __forceinline__ ContactBand contact_band(const BoxF &bx, float T) {
+    ContactBand c;
     const float m = fminf(fminf(bx.hx, bx.hy), bx.hz);
-    return m * m * (1.0f - 1e-4f) > T;  // false for NaN / zero / negative boxes as well
+    const float b1 = 2.5e-7f * __fsqrt_rn(T) * fmaxf(fmaxf(bx.bx, bx.by), bx.bz);
+    c.band = fmaf(CONTACT_QMAX + 0.5f, b1, 4e-6f * T);
+    // false for zero / negative / infinite boxes as well (a NaN component makes every wrapped estimate NaN: undecided)
+    c.ok = (m > 0.0f) && (m * m * (1.0f - 1e-4f) > T) && (c.band <= 0.25f * T);
+    return c;
 }
 __device__ __forceinline__ bool pair_contact(const float4 a, const float4 b, unsigned cb, const BoxF &bx, int pbc, float T,
-                                             bool shortcut) {
-    if (shortcut) {
+                                             const ContactBand &band) {
+    if (band.ok) {
         float dx = a.x - b.x, dy = a.y - b.y, dz = a.z - b.z;
         float qm = 0.0f;
         if (pbc && (__float_as_uint(a.w) != cb)) {
@@ -219,25 +238,29 @@ __device__ __forceinline__ bool pair_contact(const float4 a, const float4 b, uns
             qm = fmaxf(fmaxf(fabsf(qx), fabsf(qy)), fabsf(qz));
         }
         const float d2 = fmaf(dx, dx, fmaf(dy, dy, dz * dz));
-        // decided unless the estimate is within the band, not a number, or the magic rounding left its range
-        if (fabsf(d2 - T) > 4e-6f * T && qm < 2097152.0f) return d2 <= T;
+        // decided unless the estimate is within the band, not a number, or the images are QMAX or more boxes apart
+        if (fabsf(d2 - T) > band.band && qm < CONTACT_QMAX) return d2 <= T;
     }
     return pair_d2_fastwrap(a, b, cb, bx, pbc) <= T;
 }
 
 // MKB_DIST_DISTANCES_FAST: float32 distances within 4 ulp of the reference's sequence instead of its exact bits.
 // The minimum-image step keeps the reference's own roundings, w = fl(d - fl(b n)) with n = rint(d * fl(1/b)) -- so w is
-// bit-identical whenever n is the reference's roundf(fl(d/b)), and when the two integers differ (d/b within 2e-7 of a
-// half-integer) both |w| are b/2 (1 -+ 4e-7).  What is dropped: the test for that case, the unfused sum of squares
-// (two FFMA instead of four roundings) and the correctly rounded square root (MUFU.SQRT, <= 1 ulp + flush of subnormal
-// d2 to 0).  Same NaN behaviour (zero / non-finite boxes); quotients |d/b| >= 2^22 are outside the magic rounding's range.
-// 21 instead of 48 instructions per pair: the kernel becomes HBM-store bound.
+// bit-identical whenever n is the reference's roundf(fl(d/b)).  The two integers can differ only when a half-integer lies
+// between d * fl(1/b) and fl(d/b), i.e. within u |d/b| of d/b (u = 2^-24); then the two |w| are b/2 (1 -+ 2u |d/b|) and the
+// distances differ by up to 4u |d/b| relative -- a window that grows with the distance between the images (at 2^20 boxes
+// the other integer is 20 % off).  So pairs with an image integer |n| > 4 on some axis (and |d/b| >= 2^22, where the
+// magic rounding leaves its range) take the exact sequence; below, the difference stays under 1.1e-6.  What is dropped:
+// the test for the rare near-half case, the unfused sum of squares (two FFMA instead of four roundings) and the correctly
+// rounded square root (MUFU.SQRT, <= 1 ulp + flush of subnormal d2 to 0).  Same NaN behaviour (zero / non-finite boxes).
 __device__ __forceinline__ float pair_d2_quick(const float4 a, const float4 b, unsigned cb, const BoxF &bx, int pbc) {
     float dx = a.x - b.x, dy = a.y - b.y, dz = a.z - b.z;
     if (pbc && (__float_as_uint(a.w) != cb)) {
         const float nx = __fsub_rn(fmaf(dx, bx.rx, 12582912.0f), 12582912.0f);
         const float ny = __fsub_rn(fmaf(dy, bx.ry, 12582912.0f), 12582912.0f);
         const float nz = __fsub_rn(fmaf(dz, bx.rz, 12582912.0f), 12582912.0f);
+        if (fmaxf(fmaxf(fabsf(nx), fabsf(ny)), fabsf(nz)) > 4.0f)
+            return pair_d2_rewrap(dx, dy, dz, bx.bx, bx.by, bx.bz, bx.rx, bx.ry, bx.rz);
         dx = __fsub_rn(dx, __fmul_rn(bx.bx, nx));
         dy = __fsub_rn(dy, __fmul_rn(bx.by, ny));
         dz = __fsub_rn(dz, __fmul_rn(bx.bz, nz));
@@ -294,15 +317,15 @@ __global__ void MKB_K3_BOUNDS dist_kernel(const float4 *__restrict__ G1, const f
     const int rows = (int)(min(i0 + K3_ROWS, n1) - i0);
     const float4 *__restrict__ arow = G1 + f * n1 + i0;
     if (MODE == DIST_CONTACTS_D2) {  // boolean map: fused estimate + exact re-check in the band (pair_contact)
-        const bool shortcut = contact_shortcut_ok(bx, threshold);
+        const ContactBand band = contact_band(bx, threshold);
         unsigned char *const o8 = reinterpret_cast<unsigned char *>(out);
         long long idx = f * P + (SELF ? (i0 * n2 - (i0 * (i0 + 1)) / 2 + (j0 - i0 - 1)) : (i0 * n2 + j0));
         long long step = SELF ? n2 - i0 - 2 : n2;
 #pragma unroll 2
         for (int r = 0; r < rows; ++r) {
             const float4 a = __ldg(arow + r);
-            if (!SELF || j0 > i0 + r) o8[idx] = pair_contact(a, b0, cb0, bx, pbc, threshold, shortcut) ? 1 : 0;
-            if (has1 && (!SELF || j1 > i0 + r)) o8[idx + K3_COLS] = pair_contact(a, b1, cb1, bx, pbc, threshold, shortcut) ? 1 : 0;
+            if (!SELF || j0 > i0 + r) o8[idx] = pair_contact(a, b0, cb0, bx, pbc, threshold, band) ? 1 : 0;
+            if (has1 && (!SELF || j1 > i0 + r)) o8[idx + K3_COLS] = pair_contact(a, b1, cb1, bx, pbc, threshold, band) ? 1 : 0;
             idx += step;
             if (SELF) --step;
         }
