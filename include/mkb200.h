@@ -231,7 +231,9 @@ int mkb_shell_counts(mkb_handle_t h, void *stream, const mkb_traj *t, const uint
  * grid_bonds/_is_close (moleculekit/bondguesser_utils/bondguesser_utils.pyx:89-163).  coords [n,3] / radii [n] float32,
  * is_hydrogen [n] uint32, device.  pairdist = final grid box edge (after the caller's max_boxes enlargement loop).
  * Same two-call protocol as K4 with row_offsets [n + 1]; pairs come out as (i < j), unordered inside a row -- the SET
- * equals the reference's (the host wrapper returns it in canonical sorted order). */
+ * equals the reference's (the host wrapper returns it in canonical sorted order): pairs that pass _is_close AND lie in
+ * the same or adjacent boxes floor(fl32(fl32(x - xyzmin) / pairdist)) of the reference's grid on every axis, xyzmin
+ * being the per-axis minimum of coords (computed on the device). */
 int mkb_bonds_count(mkb_handle_t h, void *stream, const float *coords, const float *radii, const uint32_t *is_hydrogen,
                     int64_t n, float pairdist, int64_t *row_offsets, int64_t *total_pairs);
 int mkb_bonds_fill(mkb_handle_t h, void *stream, const float *coords, const float *radii, const uint32_t *is_hydrogen,

@@ -2,7 +2,9 @@
 
 The reference finds bonds with a uniform non-periodic cell grid built in Python (one dict insertion per atom, one
 Cython call per occupied box: moleculekit/bondguesser.py:259-392, bondguesser_utils.pyx:30-163).  Here the whole
-search runs on the GPU (csrc/bonds.cu).  The returned SET of bonds is identical to the reference's; rows come back
+search runs on the GPU (csrc/bonds.cu).  The returned SET of bonds is identical to the reference's: the pairs that pass
+its float32 ``_is_close`` test AND that its float32 box grid compares -- boxes floor((x - xyzmin) / pairdist) at most one
+apart on every axis, which two atoms pairdist apart can fail by rounding.  Rows come back
 canonical -- (min, max) pairs sorted lexicographically, the order ``calculateUniqueBonds`` produces and the
 reference's own test compares in -- rather than in the reference's box-traversal order.
 """

@@ -2,12 +2,14 @@
 //
 // Replaces moleculekit/bondguesser.py:259-392 (bond_grid_search: Python dict binning + one Cython call per occupied
 // box) and moleculekit/bondguesser_utils/bondguesser_utils.pyx:30-163 (half-shell neighbour table, _is_close,
-// grid_bonds).  The reference's result is, as a SET, every atom pair that is not H-H with
-// 0.001 <= d2 <= pairdist^2 and d2 <= (0.6 (r_i + r_j))^2, all in float32 with individually rounded operations; the
-// cell grid only prunes the search.  Here: atoms are hashed into cells of edge pairdist(1+1e-5) (count -> scan ->
-// order), one thread per atom visits the 27 neighbouring cells and keeps partners with a larger index, two passes
-// (count, cub scan, fill).  Pairs come out as (i < j); the host wrapper sorts them into the canonical order the
-// reference's own test compares in (calculateUniqueBonds).
+// grid_bonds).  The reference's result is, as a SET, every atom pair that (1) is not H-H with
+// 0.001 <= d2 <= pairdist^2 and d2 <= (0.6 (r_i + r_j))^2, all in float32 with individually rounded operations, and
+// (2) sits in the same or adjacent boxes of its float32 grid, floor(fl(fl(x - xyzmin) / pairdist)) per axis: its
+// half-shell table compares nothing further, and two rounded quotients can put atoms pairdist apart two boxes apart.
+// Here: atoms are hashed into cells of edge pairdist(1+1e-5) (count -> scan -> order), one thread per atom visits the
+// 27 neighbouring cells and keeps partners with a larger index that pass (1) and then (2) (xyzmin from one small
+// reduction), two passes (count, cub scan, fill).  Pairs come out as (i < j); the host wrapper sorts them into the
+// canonical order the reference's own test compares in (calculateUniqueBonds).
 #include <cub/device/device_scan.cuh>
 
 #include <cmath>
@@ -59,16 +61,59 @@ __device__ __forceinline__ bool bonded(const float *__restrict__ c, const float 
     return !(d2 > __fmul_rn(cut, cut));
 }
 
+// float32 -> unsigned key that decreases as the float grows (-0 just above +0), so atomicMax takes a float minimum and a
+// zeroed key lies below every finite value; key_float inverts it
+__device__ __forceinline__ unsigned min_key(float f) {
+    const unsigned u = __float_as_uint(f);
+    return (u & 0x80000000u) ? u : ~(u | 0x80000000u);
+}
+__device__ __forceinline__ float key_float(unsigned k) {
+    const unsigned t = ~k;
+    return __uint_as_float((t & 0x80000000u) ? (t & 0x7fffffffu) : ~t);
+}
+
+// the per-axis minimum of all coordinates (bondguesser.py's xyzmin) as min_key keys; key[3] starts zeroed.  Blocks of
+// 256 threads, one atomic per axis and block.
+__global__ void __launch_bounds__(256) bond_min_kernel(const float *__restrict__ coords, long long n,
+                                                       unsigned *__restrict__ key) {
+    __shared__ unsigned part[8][3];
+    unsigned m[3] = {0u, 0u, 0u};
+    for (long long a = blockIdx.x * (long long)blockDim.x + threadIdx.x; a < n; a += (long long)gridDim.x * blockDim.x)
+        for (int d = 0; d < 3; ++d) m[d] = max(m[d], min_key(coords[3 * a + d]));
+    for (int d = 0; d < 3; ++d) {
+        for (int o = 16; o; o >>= 1) m[d] = max(m[d], __shfl_xor_sync(0xffffffffu, m[d], o));
+        if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5][d] = m[d];
+    }
+    __syncthreads();
+    if (threadIdx.x < 3) {
+        unsigned v = part[0][threadIdx.x];
+        for (int w = 1; w < 8; ++w) v = max(v, part[w][threadIdx.x]);
+        atomicMax(&key[threadIdx.x], v);
+    }
+}
+
+// the reference's box of a coordinate, floor(fl32(fl32(x - xyzmin) / pairdist)): bondguesser.py bins in float32.  No
+// clamp to the box count is needed: rounding is monotone, so no atom's box exceeds that of the axis maximum.
+__device__ __forceinline__ float ref_box(float x, float mn, float pairdist) {
+    return floorf(__fdiv_rn(__fsub_rn(x, mn), pairdist));
+}
+
 template <bool FILL>
 __global__ void bond_pairs_kernel(const float *__restrict__ coords, const float *__restrict__ radii,
                                   const unsigned *__restrict__ is_h, long long n, double inv_w, float cutoff2,
-                                  unsigned hmask, const unsigned *__restrict__ bucket_start,
+                                  float pairdist, const unsigned *__restrict__ xyzmin_key, unsigned hmask,
+                                  const unsigned *__restrict__ bucket_start,
                                   const unsigned *__restrict__ order, long long *__restrict__ row_counts,
                                   const long long *__restrict__ row_offsets, unsigned *__restrict__ pairs) {
     const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (i >= n) return;
     const int cx = cell_of(coords[3 * i], inv_w), cy = cell_of(coords[3 * i + 1], inv_w),
               cz = cell_of(coords[3 * i + 2], inv_w);
+    float mn[3], box[3];
+    for (int d = 0; d < 3; ++d) {
+        mn[d] = key_float(xyzmin_key[d]);
+        box[d] = ref_box(coords[3 * i + d], mn[d], pairdist);
+    }
     long long cnt = 0, pos = FILL ? row_offsets[i] : 0;
     for (int k = 0; k < 27; ++k) {
         const int nx = cx + k / 9 - 1, ny = cy + (k / 3) % 3 - 1, nz = cz + k % 3 - 1;
@@ -80,7 +125,12 @@ __global__ void bond_pairs_kernel(const float *__restrict__ coords, const float 
             if (cell_of(coords[3 * j], inv_w) != nx || cell_of(coords[3 * j + 1], inv_w) != ny ||
                 cell_of(coords[3 * j + 2], inv_w) != nz)
                 continue;
-            if (bonded(coords, radii, is_h, i, j, cutoff2)) {
+            // the reference compares only atoms in the same or adjacent boxes of its float32 grid: two atoms pairdist
+            // apart can land two boxes apart there, and it never reports them
+            if (bonded(coords, radii, is_h, i, j, cutoff2) &&
+                fabsf(box[0] - ref_box(coords[3 * j], mn[0], pairdist)) <= 1.f &&
+                fabsf(box[1] - ref_box(coords[3 * j + 1], mn[1], pairdist)) <= 1.f &&
+                fabsf(box[2] - ref_box(coords[3 * j + 2], mn[2], pairdist)) <= 1.f) {
                 if (FILL) { pairs[2 * pos] = (unsigned)i; pairs[2 * pos + 1] = (unsigned)j; ++pos; }
                 else ++cnt;
             }
@@ -125,6 +175,16 @@ static int bond_build(mkb_ctx *h, cudaStream_t st, const float *coords, int64_t 
     MKB_CUDA(h, cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, bcount, g->bstart, (int)nb + 1, st));
     h->launches++;
     bond_order_kernel<<<gr, 256, 0, st>>>(n, ibucket, islot, g->bstart, g->order);
+    MKB_LAUNCHED(h);
+    return MKB_OK;
+}
+
+// K7 only (K10's reference tests every pair): the reference's xyzmin, for its box rule in bond_pairs_kernel
+static int bond_xyzmin(mkb_ctx *h, cudaStream_t st, const float *coords, int64_t n, unsigned **key) {
+    int rc;
+    if ((rc = scratch_get(h, S_BOND_MIN, 3, key))) return rc;
+    MKB_CUDA(h, cudaMemsetAsync(*key, 0, 3 * sizeof(unsigned), st));
+    bond_min_kernel<<<(unsigned)std::min<long long>(cdiv(n, 256), 2ll * h->sm_count), 256, 0, st>>>(coords, n, *key);
     MKB_LAUNCHED(h);
     return MKB_OK;
 }
@@ -225,10 +285,12 @@ extern "C" int mkb_bonds_count(mkb_handle_t h, void *stream, const float *coords
     if ((rc = scratch_get(h, S_ROWCNT, (size_t)n + 1, &counts))) return rc;
     if (n > 0) {
         BondGrid g;
+        unsigned *mn;
         if ((rc = bond_build(h, st, coords, n, pairdist, &g))) return rc;
+        if ((rc = bond_xyzmin(h, st, coords, n, &mn))) return rc;
         bond_pairs_kernel<false><<<(unsigned)cdiv(n, 128), 128, 0, st>>>(coords, radii, is_hydrogen, n, g.inv_w,
-                                                                         g.cutoff2, g.hmask, g.bstart, g.order, counts,
-                                                                         nullptr, nullptr);
+                                                                         g.cutoff2, pairdist, mn, g.hmask, g.bstart,
+                                                                         g.order, counts, nullptr, nullptr);
         MKB_LAUNCHED(h);
     }
     bond_set_last_zero<<<1, 32, 0, st>>>(counts, n);
@@ -257,9 +319,11 @@ extern "C" int mkb_bonds_fill(mkb_handle_t h, void *stream, const float *coords,
     if (n == 0) return MKB_OK;
     if (!row_offsets || !pairs) return fail(h, MKB_ERR_BAD_ARG, "null row_offsets/pairs");
     BondGrid g;
+    unsigned *mn;
     if ((rc = bond_build(h, st, coords, n, pairdist, &g))) return rc;
+    if ((rc = bond_xyzmin(h, st, coords, n, &mn))) return rc;
     bond_pairs_kernel<true><<<(unsigned)cdiv(n, 128), 128, 0, st>>>(coords, radii, is_hydrogen, n, g.inv_w, g.cutoff2,
-                                                                    g.hmask, g.bstart, g.order, nullptr,
+                                                                    pairdist, mn, g.hmask, g.bstart, g.order, nullptr,
                                                                     (const long long *)row_offsets, pairs);
     MKB_LAUNCHED(h);
     return MKB_OK;

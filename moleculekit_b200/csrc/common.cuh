@@ -52,6 +52,7 @@ enum ScratchSlot {
     S_XYZ_BASE,     // K26: number of the first newline of every segment
     S_XYZ_STARTS,   // K26: line starts of the staged frames
     S_XYZ_STATE,    // K26: the decode's running line count
+    S_BOND_MIN,     // K7: per-axis coordinate minimum (the reference's xyzmin) as order keys
     S_NSLOTS
 };
 

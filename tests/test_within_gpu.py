@@ -82,3 +82,29 @@ def test_device_api_large_system(oracle):
     want = np.zeros(N, bool)
     oracle.within_distance(coords, 5.0, np.arange(N, dtype=np.uint32), sel2, coords[sel2].min(0), coords[sel2].max(0), want)
     assert got.dtype == torch.bool and np.array_equal(got.cpu().numpy(), want) and 0.05 < want.mean() < 0.95
+
+
+def test_box_edge_straddles_stay_within(oracle):
+    """K10 shares K7's cell grid but its reference tests every pair: pairs pairdist apart that the bond reference's float32
+    boxes put two boxes apart (oracle/bond_grid.py) must still be found, with the cutoff just above their separation
+    (`within` compares d2 < cutoff * cutoff)."""
+    from moleculekit_b200.atomselect_utils import within_distance
+
+    from oracle import bond_grid as bg
+
+    n_miss = 0
+    for s in bg.straddle_systems(bg.STRADDLE_MINS + bg.FAR_MINS):
+        c, p = s["coords"], s["pairs"]
+        miss = bg.classify_pairs(s)[2]
+        d2 = bg.d2_f32(c[p[:, 0]], c[p[:, 1]])
+        cutoff = np.float32(np.sqrt(float(d2[miss].max() if miss.any() else d2.max())))
+        while not cutoff * cutoff > d2[miss].max(initial=0):
+            cutoff = np.nextafter(cutoff, np.float32(np.inf))
+        sel1, sel2 = p[:, 0].astype(np.uint32), p[:, 1].astype(np.uint32)
+        want, got = np.zeros(len(sel1), bool), np.zeros(len(sel1), bool)
+        mn, mx = c[sel2].min(axis=0), c[sel2].max(axis=0)
+        oracle.within_distance(c, float(cutoff), sel1, sel2, mn, mx, want)
+        within_distance(c, float(cutoff), sel1, sel2, mn, mx, got)
+        assert want[miss].all() and np.array_equal(got, want), float(s["xyzmin"])
+        n_miss += miss.sum()
+    assert n_miss >= 100
