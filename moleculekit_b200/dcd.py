@@ -321,7 +321,7 @@ def read_dcd_device(filename, frames=None, device=None, chunk_bytes: int = CHUNK
         raise _malformed("the file is empty")
     idx = index_dcd(np.memmap(filename, dtype=np.uint8, mode="r"))
     F, natoms = idx["n_frames"], idx["natoms"]
-    sel = np.arange(F, dtype=np.int64) if frames is None else np.arange(F, dtype=np.int64)[np.asarray(frames, np.int64).ravel()]
+    sel = _trajio.select(F, frames)
     info = {k: idx[k] for k in ("istart", "nsavc", "delta", "natoms", "nset", "charmm", "has_extra", "has_4d", "namnf",
                                 "title", "n_frames")}
     dev = _lib.device(device)
@@ -331,8 +331,6 @@ def read_dcd_device(filename, frames=None, device=None, chunk_bytes: int = CHUNK
         return coords, idx["box"][:, sel], idx["boxangles"][:, sel], info
     start, size, fdesc = idx["start"], idx["size"], idx["frames"]
     chunks = _trajio.chunks(sel, size, int(chunk_bytes))
-    cap = max(int(size[u].sum()) for _, _, u in chunks)
-    stream = torch.cuda.current_stream(dev)
     with open(filename, "rb") as fh:
         slot = first_buf = first = None
         if idx["free"] is not None:  # the first frame stays resident: it holds the fixed atoms of every frame
@@ -341,32 +339,21 @@ def read_dcd_device(filename, frames=None, device=None, chunk_bytes: int = CHUNK
             first = fdesc[:1].copy()
             first["offset"] -= start[0]
             slot = torch.from_numpy(_slot_map(natoms, idx["free"])).to(dev)
-        n_buf = min(2, len(chunks))
-        host = [torch.empty(cap, dtype=torch.uint8, pin_memory=True) for _ in range(n_buf)]
-        devb = [torch.empty(cap, dtype=torch.uint8, device=dev) for _ in range(n_buf)]
-        copied = [None] * n_buf
-        for c, (k0, k1, uniq) in enumerate(chunks):
-            i = c % n_buf
-            if copied[i] is not None:
-                copied[i].synchronize()  # the upload out of host[i] has left the host buffer
-            hv = host[i].numpy()
-            stage = np.concatenate([[0], np.cumsum(size[uniq])]).astype(np.int64)
-            # contiguous frames in the file are one read
-            breaks = np.flatnonzero(np.diff(uniq) != 1) + 1
-            for a, z in zip(np.concatenate([[0], breaks]), np.concatenate([breaks, [len(uniq)]])):
-                lo, nbytes = int(start[uniq[a]]), int(stage[z] - stage[a])
-                fh.seek(lo)
-                if fh.readinto(memoryview(hv)[int(stage[a]):int(stage[a]) + nbytes]) != nbytes:
-                    raise _malformed("the file changed while it was read")
-            used = int(stage[-1])
-            devb[i][:used].copy_(host[i][:used], non_blocking=True)
-            copied[i] = torch.cuda.Event()
-            copied[i].record(stream)
-            pos = np.searchsorted(uniq, sel[k0:k1])
+        staged = {}
+
+        def stage(c, host):
+            staged[c] = _trajio.stage_frames(fh.fileno(), start, size, chunks[c][2], host, "DCD")
+            return int(staged[c][-1])
+
+        def consume(c, buf):
+            k0, k1, uniq = chunks[c]
+            at = staged.pop(c)
             desc = fdesc[sel[k0:k1]].copy()
-            desc["offset"] += (stage[pos] - start[sel[k0:k1]])[:, None]
-            decode_dcd_device(devb[i][:used], desc, natoms, idx["swap"], slot, natoms - idx["namnf"], first_buf, first,
+            desc["offset"] += (at[np.searchsorted(uniq, sel[k0:k1])] - start[sel[k0:k1]])[:, None]
+            decode_dcd_device(buf, desc, natoms, idx["swap"], slot, natoms - idx["namnf"], first_buf, first,
                               out=coords[:, :, k0:k1])
+
+        _trajio.upload(dev, len(chunks), max(int(size[u].sum()) for _, _, u in chunks), stage, consume)
     return coords, idx["box"][:, sel], idx["boxangles"][:, sel], info
 
 
@@ -428,9 +415,7 @@ def encode_dcd_device(coords: torch.Tensor, box=None, boxangles=None) -> torch.T
     dev = _lib.tensor_device(coords, "encode_dcd_device")
     if coords.dtype != torch.float32:
         raise ValueError(f"coords must be float32, got {coords.dtype}")
-    box = None if box is None else np.asarray(box.cpu() if isinstance(box, torch.Tensor) else box)
-    boxangles = None if boxangles is None else \
-        np.asarray(boxangles.cpu() if isinstance(boxangles, torch.Tensor) else boxangles)
+    box, boxangles = _trajio.host(box), _trajio.host(boxangles)
     natoms, F = _writer_args(coords, box, boxangles, 0, 1, None)
     cells = None if box is None else torch.from_numpy(box_to_unitcell(box, boxangles)).to(dev)
     return _encode(coords, cells, natoms, F)
@@ -454,36 +439,37 @@ def _encode(coords, cells, natoms: int, F: int, out: torch.Tensor | None = None)
     return out[:nbytes]
 
 
-def _write(fh, coords, box, boxangles, istart, nsavc, delta, title, device, chunk_bytes) -> None:
-    if isinstance(coords, torch.Tensor):
-        if coords.dtype != torch.float32:
-            raise ValueError(f"coords must be float32, got {coords.dtype}")
-        dev = _lib.tensor_device(coords, "write_dcd")
-    else:
-        coords = np.asarray(coords, dtype=np.float32)
-        dev = None
+def _prepare(coords, box, boxangles, istart, nsavc, delta, title, device, chunk_bytes):
+    """every check, then (header, coords and unit cells as CUDA tensors or None without frames, natoms, F)"""
+    coords = _trajio.writer_coords(coords, "write_dcd")
     box = None if box is None else np.asarray(box)
     boxangles = None if boxangles is None else np.asarray(boxangles)
     natoms, F = _writer_args(coords, box, boxangles, istart, nsavc, title)
     if chunk_bytes <= 0:
         raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
-    fh.write(dcd_header(natoms, F, int(istart), int(nsavc), float(delta), title, box is not None))
+    header = dcd_header(natoms, F, int(istart), int(nsavc), float(delta), title, box is not None)
+    if F == 0:
+        return header, None, None, natoms, F
+    x = _trajio.on_device(coords, device)
+    cells = None if box is None else torch.from_numpy(box_to_unitcell(box, boxangles)).to(x.device)
+    return header, x, cells, natoms, F
+
+
+def _emit(fh, header, x, cells, natoms: int, F: int, chunk_bytes) -> None:
+    fh.write(header)
     if F == 0:
         return
-    if dev is None:
-        dev = _lib.device(device)
-        coords = torch.from_numpy(np.ascontiguousarray(coords)).to(dev)
-    cells = None if box is None else torch.from_numpy(box_to_unitcell(box, boxangles)).to(dev)
-    _trajio.write_encoded(fh, dev, F, _frame_bytes(natoms, cells is not None), chunk_bytes,
-                          lambda f0, f1, out: _encode(coords[:, :, f0:f1], None if cells is None else cells[f0:f1],
-                                                      natoms, f1 - f0, out=out))
+    _trajio.write_encoded(fh, x.device, F, _frame_bytes(natoms, cells is not None), chunk_bytes,
+                          lambda f0, f1, out: _encode(x[:, :, f0:f1], None if cells is None else cells[f0:f1], natoms,
+                                                      f1 - f0, out=out))
 
 
 def dcd_bytes(coords, box=None, boxangles=None, istart: int = 0, nsavc: int = 1, delta: float = 1.0, title=None,
               device=None, chunk_bytes: int = CHUNK_BYTES) -> bytes:
     """The file :func:`write_dcd` writes, as a ``bytes`` object."""
+    prep = _prepare(coords, box, boxangles, istart, nsavc, delta, title, device, chunk_bytes)
     fh = io.BytesIO()
-    _write(fh, coords, box, boxangles, istart, nsavc, delta, title, device, chunk_bytes)
+    _emit(fh, *prep, chunk_bytes)
     return fh.getvalue()
 
 
@@ -497,11 +483,6 @@ def write_dcd(filename, coords, box=None, boxangles=None, istart: int = 0, nsavc
     arguments are checked before it is opened."""
     if isinstance(filename, bytes):
         filename = filename.decode("UTF-8")
-    if isinstance(coords, torch.Tensor):
-        _lib.tensor_device(coords, "write_dcd")
-    else:
-        coords = np.asarray(coords, dtype=np.float32)
-    _writer_args(coords, None if box is None else np.asarray(box), None if boxangles is None else np.asarray(boxangles),
-                 istart, nsavc, title)
+    prep = _prepare(coords, box, boxangles, istart, nsavc, delta, title, device, chunk_bytes)
     with open(filename, "wb") as fh:
-        _write(fh, coords, box, boxangles, istart, nsavc, delta, title, device, chunk_bytes)
+        _emit(fh, *prep, chunk_bytes)

@@ -170,8 +170,8 @@ def _malformed(filename, idx, natoms: int, frame: int, b: int) -> ValueError:
                       f"{'with' if idx['has_box'] else 'no'} box line), line {line}, column {col + 1}: {what}")
 
 
-def _read(filename, natoms, select, box, device, chunk_bytes):
-    """The frames ``select(n_frames)`` picks -> (coords CUDA (natoms, 3, F), box (3, F) numpy, info)"""
+def _read(filename, natoms, frames, box, device, chunk_bytes):
+    """The frames :func:`_trajio.select` picks -> (coords CUDA (natoms, 3, F), box (3, F) numpy, info)"""
     if isinstance(filename, bytes):
         filename = filename.decode("UTF-8")
     if chunk_bytes <= 0:
@@ -180,7 +180,7 @@ def _read(filename, natoms, select, box, device, chunk_bytes):
     mm = np.memmap(filename, dtype=np.uint8, mode="r") if os.path.getsize(filename) else b""
     idx = index_mdcrd(mm, natoms, box)
     F, S, hb = idx["n_frames"], idx["frame_bytes"], idx["has_box"]
-    sel = select(F)
+    sel = _trajio.select(F, frames)
     info = dict(title=idx["title"], has_box=hb, natoms=natoms, n_frames=F, frames=sel)
     dev = _lib.device(device)
     n = len(sel)
@@ -190,27 +190,22 @@ def _read(filename, natoms, select, box, device, chunk_bytes):
     del mm  # the frames are read with preadv: a copy from the page cache, without a page fault per 4 KiB
     row = (S + 15) & ~15  # every staged frame starts on a 16-byte boundary
     chunks = _trajio.chunks(sel, np.full(F, row, np.int64), int(chunk_bytes))
-    cap = max(len(u) for _, _, u in chunks) * row
     box_d = torch.zeros((3, n), dtype=torch.float32, device=dev)
     bad = torch.full((len(chunks),), INT64_MAX, dtype=torch.int64, device=dev)  # one slot per chunk: no sync per chunk
-    stream = torch.cuda.current_stream(dev)
-    n_buf = min(2, len(chunks))
-    host = [torch.empty(cap, dtype=torch.uint8, pin_memory=True) for _ in range(n_buf)]
-    devb = [torch.empty(cap, dtype=torch.uint8, device=dev) for _ in range(n_buf)]
-    copied = [None] * n_buf
     with open(filename, "rb") as fh:
-        for c, (k0, k1, uniq) in enumerate(chunks):
-            i = c % n_buf
-            if copied[i] is not None:
-                copied[i].synchronize()  # the upload out of host[i] has left the host buffer
+        def stage(c, host):
+            uniq = chunks[c][2]
             used = len(uniq) * row
-            rows = host[i].numpy()[:used].reshape(len(uniq), row)[:, :S]
+            rows = host[:used].reshape(len(uniq), row)[:, :S]
             _trajio.gather_slabs(fh.fileno(), idx["offset"] + uniq * S, S, rows, "AMBER mdcrd")
-            devb[i][:used].copy_(host[i][:used], non_blocking=True)
-            copied[i] = torch.cuda.Event()
-            copied[i].record(stream)
-            decode_mdcrd_device(devb[i][:used], np.searchsorted(uniq, sel[k0:k1]) * row, natoms, hb,
-                                out=coords[:, :, k0:k1], box_out=box_d[:, k0:k1] if hb else None, bad=bad[c:c + 1])
+            return used
+
+        def consume(c, buf):
+            k0, k1, uniq = chunks[c]
+            decode_mdcrd_device(buf, np.searchsorted(uniq, sel[k0:k1]) * row, natoms, hb, out=coords[:, :, k0:k1],
+                                box_out=box_d[:, k0:k1] if hb else None, bad=bad[c:c + 1])
+
+        _trajio.upload(dev, len(chunks), max(len(u) for _, _, u in chunks) * row, stage, consume)
     worst = bad.cpu().numpy()
     box_h = box_d.cpu().numpy()
     hit = np.flatnonzero(worst != INT64_MAX)
@@ -221,14 +216,6 @@ def _read(filename, natoms, select, box, device, chunk_bytes):
     return coords, box_h, info
 
 
-def _select(frames):
-    def select(F):
-        if frames is None:
-            return np.arange(F, dtype=np.int64)
-        return np.arange(F, dtype=np.int64)[np.asarray(frames, np.int64).ravel()]
-    return select
-
-
 def read_mdcrd_device(filename, natoms: int, frames=None, box: bool | None = None, device=None,
                       chunk_bytes: int = CHUNK_BYTES):
     """Every frame (or the frames listed in ``frames``: any order, repeats allowed; out of range raises IndexError) ->
@@ -237,19 +224,19 @@ def read_mdcrd_device(filename, natoms: int, frames=None, box: bool | None = Non
     holds title, has_box, natoms, n_frames (frames in the file) and frames (the file frame of each returned frame).
     A malformed field or a misplaced newline raises ValueError naming the frame, the 1-based line and column and the
     field's bytes."""
-    return _read(filename, natoms, _select(frames), box, device, chunk_bytes)
+    return _read(filename, natoms, frames, box, device, chunk_bytes)
 
 
 def read_mdcrd(filename, natoms: int, box: bool | None = None, device=None, chunk_bytes: int = CHUNK_BYTES):
     """Every frame -> (coords (natoms, 3, F) float32 [Angstrom], box (3, F) float32) as numpy arrays."""
-    coords, bx, _ = _read(filename, natoms, _select(None), box, device, chunk_bytes)
+    coords, bx, _ = _read(filename, natoms, None, box, device, chunk_bytes)
     return coords.cpu().numpy(), bx
 
 
 def read_mdcrd_frames(filename, natoms: int, frames, box: bool | None = None, device=None,
                       chunk_bytes: int = CHUNK_BYTES):
     """:func:`read_mdcrd` for the listed frames (any order, repeats allowed; out of range raises IndexError)."""
-    coords, bx, _ = _read(filename, natoms, _select(frames), box, device, chunk_bytes)
+    coords, bx, _ = _read(filename, natoms, frames, box, device, chunk_bytes)
     return coords.cpu().numpy(), bx
 
 
@@ -269,8 +256,6 @@ def _writer_args(coords, box, title, chunk_bytes):
     natoms, _, F = (int(v) for v in coords.shape)
     if not 1 <= natoms <= MAX_ATOMS:
         raise ValueError(f"an mdcrd frame written here holds 1 to {MAX_ATOMS} atoms, got {natoms}")
-    if isinstance(coords, torch.Tensor) and coords.dtype != torch.float32:
-        raise ValueError(f"coords must be float32, got {coords.dtype}")
     if box is not None:
         if tuple(box.shape) != (3, F):
             raise ValueError(f"box must be (3, F) = {(3, F)}, got {tuple(box.shape)}")
@@ -315,11 +300,7 @@ def _check_range(a, name: str) -> None:
 
 def _prepare(coords, box, title, device, chunk_bytes):
     """every check, then (coords, box) as CUDA tensors (a CUDA tensor used where it is, numpy uploaded), natoms, F"""
-    if isinstance(coords, torch.Tensor):
-        dev = _lib.tensor_device(coords, "write_mdcrd")
-    else:
-        coords = np.asarray(coords, dtype=np.float32)
-        dev = None
+    coords = _trajio.writer_coords(coords, "write_mdcrd")
     if box is not None and not isinstance(box, torch.Tensor):
         box = np.asarray(box, dtype=np.float32)
     natoms, F = _writer_args(coords, box, title, chunk_bytes)
@@ -328,12 +309,10 @@ def _prepare(coords, box, title, device, chunk_bytes):
         _check_range(box, "box")
     if F == 0:
         return None, None, natoms, F
-    if dev is None:
-        dev = _lib.device(device)
-        coords = torch.from_numpy(np.ascontiguousarray(coords)).to(dev)
+    x = _trajio.on_device(coords, device)
     if box is not None:
-        box = box.to(dev) if isinstance(box, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(box)).to(dev)
-    return coords, box, natoms, F
+        box = box.to(x.device) if isinstance(box, torch.Tensor) else _trajio.on_device(box, x.device)
+    return x, box, natoms, F
 
 
 def _encode(x, box, natoms: int, F: int, out: torch.Tensor | None = None) -> torch.Tensor:

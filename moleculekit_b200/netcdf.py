@@ -279,11 +279,6 @@ def decode_netcdf_device(buf: torch.Tensor, offsets, natoms: int, out: torch.Ten
     return out
 
 
-def _gather_slabs(fd: int, starts: np.ndarray, slab: int, out: np.ndarray) -> None:
-    """:func:`_trajio.gather_slabs` for a NetCDF file"""
-    _trajio.gather_slabs(fd, starts, slab, out, "NetCDF")
-
-
 def read_netcdf_device(filename, frames=None, device=None, chunk_bytes: int = CHUNK_BYTES):
     """Whole file (or the frames listed: any order, repeats allowed; out of range raises IndexError) -> (coords CUDA
     (natoms, 3, F) float32 [Angstrom], box (3, F) float32, boxangles (3, F) float32, info dict) with the trajectory left
@@ -299,7 +294,7 @@ def read_netcdf_device(filename, frames=None, device=None, chunk_bytes: int = CH
     mm = np.memmap(filename, dtype=np.uint8, mode="r")
     idx = index_netcdf(mm)
     F, natoms = idx["n_frames"], idx["natoms"]
-    sel = np.arange(F, dtype=np.int64) if frames is None else np.arange(F, dtype=np.int64)[np.asarray(frames, np.int64).ravel()]
+    sel = _trajio.select(F, frames)
     info = {k: idx[k] for k in ("natoms", "n_frames", "numrecs", "version", "title", "application", "program",
                                 "programVersion", "Conventions", "ConventionVersion")}
     info["time"] = idx["time"][sel]
@@ -311,25 +306,19 @@ def read_netcdf_device(filename, frames=None, device=None, chunk_bytes: int = CH
     del mm  # the slabs are read with preadv: a copy from the page cache, without a page fault per 4 KiB
     slab = 12 * natoms
     chunks = _trajio.chunks(sel, np.full(F, slab, np.int64), int(chunk_bytes))
-    cap = max(len(u) for _, _, u in chunks) * slab
-    stream = torch.cuda.current_stream(dev)
-    n_buf = min(2, len(chunks))
-    host = [torch.empty(cap, dtype=torch.uint8, pin_memory=True) for _ in range(n_buf)]
-    devb = [torch.empty(cap, dtype=torch.uint8, device=dev) for _ in range(n_buf)]
-    copied = [None] * n_buf
     with open(filename, "rb") as fh:
-        for c, (k0, k1, uniq) in enumerate(chunks):
-            i = c % n_buf
-            if copied[i] is not None:
-                copied[i].synchronize()  # the upload out of host[i] has left the host buffer
+        def stage(c, host):
+            uniq = chunks[c][2]
             used = len(uniq) * slab
-            _gather_slabs(fh.fileno(), idx["begin"] + uniq * idx["recsize"], slab,
-                          host[i].numpy()[:used].reshape(len(uniq), slab))
-            devb[i][:used].copy_(host[i][:used], non_blocking=True)
-            copied[i] = torch.cuda.Event()
-            copied[i].record(stream)
-            decode_netcdf_device(devb[i][:used], np.searchsorted(uniq, sel[k0:k1]) * slab, natoms,
-                                 out=coords[:, :, k0:k1])
+            _trajio.gather_slabs(fh.fileno(), idx["begin"] + uniq * idx["recsize"], slab,
+                                 host[:used].reshape(len(uniq), slab), "NetCDF")
+            return used
+
+        def consume(c, buf):
+            k0, k1, uniq = chunks[c]
+            decode_netcdf_device(buf, np.searchsorted(uniq, sel[k0:k1]) * slab, natoms, out=coords[:, :, k0:k1])
+
+        _trajio.upload(dev, len(chunks), max(len(u) for _, _, u in chunks) * slab, stage, consume)
     return coords, idx["box"][:, sel], idx["boxangles"][:, sel], info
 
 
@@ -427,10 +416,6 @@ def _writer_args(coords, box, boxangles, time, title):
     return natoms, F
 
 
-def _host(v):
-    return None if v is None else np.asarray(v.cpu() if isinstance(v, torch.Tensor) else v)
-
-
 def _extra(F: int, box, boxangles, time) -> np.ndarray:
     """(F, 4 or 52) uint8: each record's time, cell_lengths and cell_angles in file byte order"""
     e = np.zeros(F, EXTRA_NOBOX if box is None else EXTRA_BOX)
@@ -462,42 +447,44 @@ def encode_netcdf_device(coords: torch.Tensor, box=None, boxangles=None, time=No
     dev = _lib.tensor_device(coords, "encode_netcdf_device")
     if coords.dtype != torch.float32:
         raise ValueError(f"coords must be float32, got {coords.dtype}")
-    box, boxangles, time = _host(box), _host(boxangles), _host(time)
+    box, boxangles, time = _trajio.host(box), _trajio.host(boxangles), _trajio.host(time)
     natoms, F = _writer_args(coords, box, boxangles, time, None)
     extra = torch.from_numpy(_extra(F, box, boxangles, time)).to(dev)
     return _encode(coords, extra, natoms, F, box is not None)
 
 
-def _write(fh, coords, box, boxangles, time, title, device, chunk_bytes) -> None:
-    if isinstance(coords, torch.Tensor):
-        if coords.dtype != torch.float32:
-            raise ValueError(f"coords must be float32, got {coords.dtype}")
-        dev = _lib.tensor_device(coords, "write_netcdf")
-    else:
-        coords = np.asarray(coords, dtype=np.float32)
-        dev = None
-    box, boxangles, time = _host(box), _host(boxangles), _host(time)
+def _prepare(coords, box, boxangles, time, title, device, chunk_bytes):
+    """every check, then (header, coords and the host-built record bytes as CUDA tensors or None without frames,
+    natoms, F, with_box)"""
+    coords = _trajio.writer_coords(coords, "write_netcdf")
+    box, boxangles, time = _trajio.host(box), _trajio.host(boxangles), _trajio.host(time)
     natoms, F = _writer_args(coords, box, boxangles, time, title)
     if chunk_bytes <= 0:
         raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
-    fh.write(netcdf_header(natoms, F, box is not None, title))
+    with_box = box is not None
+    header = netcdf_header(natoms, F, with_box, title)
+    if F == 0:
+        return header, None, None, natoms, F, with_box
+    x = _trajio.on_device(coords, device)
+    extra = torch.from_numpy(_extra(F, box, boxangles, time)).to(x.device)
+    return header, x, extra, natoms, F, with_box
+
+
+def _emit(fh, header, x, extra, natoms: int, F: int, with_box: bool, chunk_bytes) -> None:
+    fh.write(header)
     if F == 0:
         return
-    if dev is None:
-        dev = _lib.device(device)
-        coords = torch.from_numpy(np.ascontiguousarray(coords)).to(dev)
-    extra = torch.from_numpy(_extra(F, box, boxangles, time)).to(dev)
-    with_box = box is not None
-    _trajio.write_encoded(fh, dev, F, _record_layout(natoms, with_box)[0], chunk_bytes,
-                          lambda f0, f1, out: _encode(coords[:, :, f0:f1], extra[f0:f1], natoms, f1 - f0, with_box,
+    _trajio.write_encoded(fh, x.device, F, _record_layout(natoms, with_box)[0], chunk_bytes,
+                          lambda f0, f1, out: _encode(x[:, :, f0:f1], extra[f0:f1], natoms, f1 - f0, with_box,
                                                       out=out))
 
 
 def netcdf_bytes(coords, box=None, boxangles=None, time=None, title=None, device=None,
                  chunk_bytes: int = CHUNK_BYTES) -> bytes:
     """The file :func:`write_netcdf` writes, as a ``bytes`` object."""
+    prep = _prepare(coords, box, boxangles, time, title, device, chunk_bytes)
     fh = io.BytesIO()
-    _write(fh, coords, box, boxangles, time, title, device, chunk_bytes)
+    _emit(fh, *prep, chunk_bytes)
     return fh.getvalue()
 
 
@@ -512,12 +499,6 @@ def write_netcdf(filename, coords, box=None, boxangles=None, time=None, title=No
     created or truncated; arguments are checked before it is opened."""
     if isinstance(filename, bytes):
         filename = filename.decode("UTF-8")
-    if isinstance(coords, torch.Tensor):
-        _lib.tensor_device(coords, "write_netcdf")
-    else:
-        coords = np.asarray(coords, dtype=np.float32)
-    _writer_args(coords, _host(box), _host(boxangles), _host(time), title)
-    if chunk_bytes <= 0:
-        raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
+    prep = _prepare(coords, box, boxangles, time, title, device, chunk_bytes)
     with open(filename, "wb") as fh:
-        _write(fh, coords, box, boxangles, time, title, device, chunk_bytes)
+        _emit(fh, *prep, chunk_bytes)

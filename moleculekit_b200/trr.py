@@ -201,26 +201,21 @@ def _read(filename, select, fields, scale, device, chunk_bytes):
     order = [f for f in FIELDS if f in fields]  # file order: ascending offsets within a record
     nf = len(order)
     chunks = _trajio.chunks(sel, np.full(R, nf * slab, np.int64), int(chunk_bytes))
-    cap = max(len(u) for _, _, u in chunks) * nf * slab
-    stream = torch.cuda.current_stream(dev)
-    n_buf = min(2, len(chunks))
-    host = [torch.empty(cap, dtype=torch.uint8, pin_memory=True) for _ in range(n_buf)]
-    devb = [torch.empty(cap, dtype=torch.uint8, device=dev) for _ in range(n_buf)]
-    copied = [None] * n_buf
     with open(filename, "rb") as fh:
-        for c, (k0, k1, uniq) in enumerate(chunks):
-            i = c % n_buf
-            if copied[i] is not None:
-                copied[i].synchronize()  # the upload out of host[i] has left the host buffer
+        def stage(c, host):
+            uniq = chunks[c][2]
             used = len(uniq) * nf * slab
             starts = np.stack([idx[f"{f}_offset"][uniq] for f in order], axis=1).reshape(-1)
-            _trajio.gather_slabs(fh.fileno(), starts, slab, host[i].numpy()[:used].reshape(len(uniq) * nf, slab), "TRR")
-            devb[i][:used].copy_(host[i][:used], non_blocking=True)
-            copied[i] = torch.cuda.Event()
-            copied[i].record(stream)
+            _trajio.gather_slabs(fh.fileno(), starts, slab, host[:used].reshape(len(uniq) * nf, slab), "TRR")
+            return used
+
+        def consume(c, buf):
+            k0, k1, uniq = chunks[c]
             row = np.searchsorted(uniq, sel[k0:k1]) * nf
             for j, f in enumerate(order):
-                decode_trr_device(devb[i][:used], (row + j) * slab, natoms, w, out=out[f][:, :, k0:k1])
+                decode_trr_device(buf, (row + j) * slab, natoms, w, out=out[f][:, :, k0:k1])
+
+        _trajio.upload(dev, len(chunks), max(len(u) for _, _, u in chunks) * nf * slab, stage, consume)
     s = np.float32(scale)
     if "x" in out and s != 1:
         out["x"].mul_(float(s))  # one float32 multiply of the rounded value
@@ -244,7 +239,7 @@ def read_trr_device(filename, frames=None, fields=("x",), scale: float = 1.0, de
             for f in _fields(fields):
                 have &= idx[f"has_{f}"]
             return np.flatnonzero(have).astype(np.int64)
-        return np.arange(R, dtype=np.int64)[np.asarray(frames, np.int64).ravel()]
+        return _trajio.select(R, frames)
 
     return _read(filename, select, fields, scale, device, chunk_bytes)
 
@@ -266,10 +261,6 @@ def read_trr_frames(filename, frames, device=None, chunk_bytes: int = CHUNK_BYTE
 
 
 # ------------------------------------------------------------------------------------------------------------ writing
-def _host(v):
-    return None if v is None else np.asarray(v.cpu() if isinstance(v, torch.Tensor) else v)
-
-
 def _writer_args(coords, box, time, step, lambd, velocities, forces, scale, chunk_bytes):
     """shapes and values checked before any device work; returns (natoms, F)"""
     if coords.ndim != 3 or coords.shape[1] != 3:
@@ -313,13 +304,6 @@ def _heads(natoms: int, F: int, box, time, step, lambd, with_v: bool, with_f: bo
     return h.view(np.uint8).reshape(F, HEAD.itemsize)
 
 
-def _on(v, dev):
-    """a (natoms, 3, F) float32 array on ``dev``: a CUDA tensor as it is, a numpy array uploaded"""
-    if v is None or isinstance(v, torch.Tensor):
-        return v
-    return torch.from_numpy(np.ascontiguousarray(v, dtype=np.float32)).to(dev)
-
-
 def _encode(x, v, f, head, natoms: int, F: int, out: torch.Tensor | None = None) -> torch.Tensor:
     dev = x.device
     arrs = [_trajio.frame_minor(a) for a in (x, v, f) if a is not None]
@@ -346,36 +330,39 @@ def encode_trr_device(coords: torch.Tensor, box, time, step, lambd=None, velocit
     """K24 on the device: ``coords`` (CUDA (natoms, 3, F) float32, frame-minor; a frame slice of a larger tensor is
     used in place) -> uint8 CUDA tensor of the F records of :func:`write_trr`'s file back to back."""
     dev = _lib.tensor_device(coords, "encode_trr_device")
-    box, time, step, lambd = _host(box), _host(time), _host(step), _host(lambd)
+    box, time, step, lambd = (_trajio.host(a) for a in (box, time, step, lambd))
     natoms, F = _writer_args(coords, box, time, step, lambd, velocities, forces, scale, 1)
     head = torch.from_numpy(_heads(natoms, F, box, time, step, lambd, velocities is not None,
                                    forces is not None)).to(dev)
-    return _encode(_scaled(coords, scale), _on(velocities, dev), _on(forces, dev), head, natoms, F)
+    return _encode(_scaled(coords, scale), _trajio.on_device(velocities, dev), _trajio.on_device(forces, dev), head,
+                   natoms, F)
 
 
-def _write(fh, coords, box, time, step, lambd, velocities, forces, scale, device, chunk_bytes) -> None:
-    if isinstance(coords, torch.Tensor):
-        dev = _lib.tensor_device(coords, "write_trr")
-    else:
-        coords = np.asarray(coords, dtype=np.float32)
-        dev = None
-    box, time, step, lambd = _host(box), _host(time), _host(step), _host(lambd)
+def _prepare(coords, box, time, step, lambd, velocities, forces, scale, device, chunk_bytes):
+    """every check, then (x, v, f and the host-built headers as CUDA tensors or None without frames, natoms, F)"""
+    coords = _trajio.writer_coords(coords, "write_trr")
+    box, time, step, lambd = (_trajio.host(a) for a in (box, time, step, lambd))
     natoms, F = _writer_args(coords, box, time, step, lambd, velocities, forces, scale, chunk_bytes)
     if F == 0:
-        return
-    if dev is None:
-        dev = _lib.device(device)
-    x, v, f = _scaled(_on(coords, dev), scale), _on(velocities, dev), _on(forces, dev)
-    for name, a in (("velocities", v), ("forces", f)):
-        if a is not None and a.device != dev:
+        return None, None, None, None, natoms, F
+    dev = coords.device if isinstance(coords, torch.Tensor) else _lib.device(device)
+    for name, a in (("velocities", velocities), ("forces", forces)):
+        if isinstance(a, torch.Tensor) and a.device != dev:
             raise ValueError(f"{name} are on {a.device}, coords on {dev}")
+    x, v, f = (_trajio.on_device(a, dev) for a in (coords, velocities, forces))
     head = torch.from_numpy(_heads(natoms, F, box, time, step, lambd, v is not None, f is not None)).to(dev)
+    return _scaled(x, scale), v, f, head, natoms, F
+
+
+def _emit(fh, x, v, f, head, natoms: int, F: int, chunk_bytes) -> None:
+    if F == 0:
+        return
     record_bytes = HEAD.itemsize + 12 * natoms * (1 + (v is not None) + (f is not None))
 
     def part(a, f0, f1):
         return None if a is None else a[:, :, f0:f1]
 
-    _trajio.write_encoded(fh, dev, F, record_bytes, chunk_bytes,
+    _trajio.write_encoded(fh, x.device, F, record_bytes, chunk_bytes,
                           lambda f0, f1, out: _encode(x[:, :, f0:f1], part(v, f0, f1), part(f, f0, f1), head[f0:f1],
                                                       natoms, f1 - f0, out=out))
 
@@ -383,8 +370,9 @@ def _write(fh, coords, box, time, step, lambd, velocities, forces, scale, device
 def trr_bytes(coords, box, time, step, lambd=None, velocities=None, forces=None, scale: float = 1.0, device=None,
               chunk_bytes: int = CHUNK_BYTES) -> bytes:
     """The file :func:`write_trr` writes, as a ``bytes`` object."""
+    prep = _prepare(coords, box, time, step, lambd, velocities, forces, scale, device, chunk_bytes)
     fh = io.BytesIO()
-    _write(fh, coords, box, time, step, lambd, velocities, forces, scale, device, chunk_bytes)
+    _emit(fh, *prep, chunk_bytes)
     return fh.getvalue()
 
 
@@ -400,10 +388,6 @@ def write_trr(filename, coords, box, time, step, lambd=None, velocities=None, fo
     arguments are checked before it is opened."""
     if isinstance(filename, bytes):
         filename = filename.decode("UTF-8")
-    if isinstance(coords, torch.Tensor):
-        _lib.tensor_device(coords, "write_trr")
-    else:
-        coords = np.asarray(coords, dtype=np.float32)
-    _writer_args(coords, _host(box), _host(time), _host(step), _host(lambd), velocities, forces, scale, chunk_bytes)
+    prep = _prepare(coords, box, time, step, lambd, velocities, forces, scale, device, chunk_bytes)
     with open(filename, "wb") as fh:
-        _write(fh, coords, box, time, step, lambd, velocities, forces, scale, device, chunk_bytes)
+        _emit(fh, *prep, chunk_bytes)

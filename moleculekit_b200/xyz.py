@@ -55,15 +55,6 @@ def _name(filename) -> str:
     return filename.decode("UTF-8") if isinstance(filename, bytes) else str(filename)
 
 
-def _pread_full(fd: int, buf: memoryview, pos: int) -> None:
-    done = 0
-    while done < len(buf):
-        got = os.preadv(fd, [buf[done:done + _trajio.PREADV_BYTES]], pos + done)
-        if got <= 0:
-            raise RuntimeError("Malformed XYZ file: the file changed while it was read")
-        done += got
-
-
 def _content_end(fd: int, size: int) -> int:
     """one past the last byte that is not ASCII whitespace (0 for a blank file)"""
     end, step = size, 1 << 16
@@ -186,24 +177,17 @@ def index_xyz(filename, device=None, chunk_bytes: int = CHUNK_BYTES) -> dict:
         state = torch.tensor([0, INT64_MAX, 0], dtype=torch.int64, device=dev)
         frame_off = torch.zeros(cap + 1, dtype=torch.int64, device=dev)  # + 1: the end of the last frame, set below
         status = torch.zeros(cap, dtype=torch.uint8, device=dev)
-        starts = list(range(0, E, B))
-        n_buf = min(2, len(starts))
-        size = min(B, E) + LOOKAHEAD + 16
-        host = [torch.empty(size, dtype=torch.uint8, pin_memory=True) for _ in range(n_buf)]
-        devb = [torch.empty(size, dtype=torch.uint8, device=dev) for _ in range(n_buf)]
-        copied = [None] * n_buf
-        stream = torch.cuda.current_stream(dev)
-        for c, c0 in enumerate(starts):
-            i = c % n_buf
-            if copied[i] is not None:
-                copied[i].synchronize()  # the upload out of host[i] has left the host buffer
-            n, n_read = min(B, E - c0), min(B + LOOKAHEAD, E - c0)
-            _pread_full(fd, memoryview(host[i].numpy())[:n_read], c0)
-            devb[i][:n_read].copy_(host[i][:n_read], non_blocking=True)
-            copied[i] = torch.cuda.Event()
-            copied[i].record(stream)
-            _lib.call(dev, "mkb_xyz_index", _lib.ptr(devb[i]), n, n_read, c0, natoms, _lib.ptr(state),
-                      _lib.ptr(frame_off), _lib.ptr(status), cap)
+
+        def stage(c, host):
+            n_read = min(B + LOOKAHEAD, E - c * B)
+            _trajio.read_exact(fd, host[:n_read], c * B, "XYZ")
+            return n_read
+
+        def consume(c, buf):
+            _lib.call(dev, "mkb_xyz_index", _lib.ptr(buf), min(B, E - c * B), int(buf.numel()), c * B, natoms,
+                      _lib.ptr(state), _lib.ptr(frame_off), _lib.ptr(status), cap)
+
+        _trajio.upload(dev, -(-E // B), min(B, E) + LOOKAHEAD, stage, consume)
         lines, lone_cr, past = (int(v) for v in state.cpu())
         lines += 1  # the last line ends at E, without a newline
         F, rest = divmod(lines, P)
@@ -275,28 +259,13 @@ def decode_xyz_device(buf: torch.Tensor, n_staged: int, frame_of, natoms: int, o
     return out, flags
 
 
-def _stage(fd: int, offsets: np.ndarray, uniq: np.ndarray, host: torch.Tensor) -> int:
-    """read the frames ``uniq`` (ascending) back to back into ``host``; runs of consecutive frames in one read each"""
-    mv = memoryview(host.numpy())
-    at, k = 0, 0
-    while k < len(uniq):
-        j = k
-        while j + 1 < len(uniq) and uniq[j + 1] == uniq[j] + 1:
-            j += 1
-        lo, hi = int(offsets[uniq[k]]), int(offsets[uniq[j] + 1])
-        _pread_full(fd, mv[at:at + hi - lo], lo)
-        at += hi - lo
-        k = j + 1
-    return at
-
-
-def _read(filename, select, index, device, chunk_bytes):
+def _read(filename, frames, index, device, chunk_bytes):
     fn = _name(filename)
     if chunk_bytes <= 0:
         raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
     idx = index if index is not None else index_xyz(fn, device, chunk_bytes)
     N, F, offs = int(idx["natoms"]), int(idx["n_frames"]), np.asarray(idx["offsets"], np.int64)
-    sel = select(F)
+    sel = _trajio.select(F, frames)
     dev = _lib.device(device)
     n = len(sel)
     coords = torch.empty((N, 3, n), dtype=torch.float32, device=dev)
@@ -305,25 +274,19 @@ def _read(filename, select, index, device, chunk_bytes):
         return coords, info
     sizes = np.diff(offs)
     chunks = _trajio.chunks(sel, sizes, int(chunk_bytes))
-    cap = max(int(sizes[u].sum()) for _, _, u in chunks) + 16
     flags = torch.zeros(1 + 2 * FLAG_CAP, dtype=torch.int64, device=dev)
-    stream = torch.cuda.current_stream(dev)
-    n_buf = min(2, len(chunks))
-    host = [torch.empty(cap, dtype=torch.uint8, pin_memory=True) for _ in range(n_buf)]
-    devb = [torch.empty(cap, dtype=torch.uint8, device=dev) for _ in range(n_buf)]
-    copied = [None] * n_buf
     with open(fn, "rb") as fh:
         fd = fh.fileno()
-        for c, (k0, k1, uniq) in enumerate(chunks):
-            i = c % n_buf
-            if copied[i] is not None:
-                copied[i].synchronize()  # the upload out of host[i] has left the host buffer
-            used = _stage(fd, offs, uniq, host[i])
-            devb[i][:used].copy_(host[i][:used], non_blocking=True)
-            copied[i] = torch.cuda.Event()
-            copied[i].record(stream)
-            decode_xyz_device(devb[i][:used], len(uniq), np.searchsorted(uniq, sel[k0:k1]), N,
-                              out=coords[:, :, k0:k1], flags=flags, frame_base=k0)
+
+        def stage(c, host):
+            return int(_trajio.stage_frames(fd, offs[:-1], sizes, chunks[c][2], host, "XYZ")[-1])
+
+        def consume(c, buf):
+            k0, k1, uniq = chunks[c]
+            decode_xyz_device(buf, len(uniq), np.searchsorted(uniq, sel[k0:k1]), N, out=coords[:, :, k0:k1],
+                              flags=flags, frame_base=k0)
+
+        _trajio.upload(dev, len(chunks), max(int(sizes[u].sum()) for _, _, u in chunks), stage, consume)
         n_host = int(flags[0].item())
         if n_host:
             if n_host <= FLAG_CAP:
@@ -356,32 +319,24 @@ def _host_lines(fn, fd, offs, sel, N, k, a, rel, coords) -> None:
     coords[torch.from_numpy(a).to(dev), :, torch.from_numpy(k).to(dev)] = torch.from_numpy(vals).to(dev)
 
 
-def _select(frames):
-    def select(F):
-        if frames is None:
-            return np.arange(F, dtype=np.int64)
-        return np.arange(F, dtype=np.int64)[np.asarray(frames, np.int64).ravel()]
-    return select
-
-
 def read_xyz_device(filename, frames=None, index: dict | None = None, device=None, chunk_bytes: int = CHUNK_BYTES):
     """Every frame (or the frames listed in ``frames``: any order, repeats allowed; out of range raises IndexError) ->
     (coords CUDA (natoms, 3, F) float32 [Angstrom], info) with the trajectory left on the GPU.  ``index`` (what
     :func:`index_xyz` returned for this file) skips the index pass.  ``info`` holds natoms, n_frames (frames in the
     file), frames (the file frame of each returned frame), element and comment (frame 0's) and host_lines (the atom
     lines re-read on the host).  Errors: see the module docstring."""
-    return _read(filename, _select(frames), index, device, chunk_bytes)
+    return _read(filename, frames, index, device, chunk_bytes)
 
 
 def read_xyz(filename, index: dict | None = None, device=None, chunk_bytes: int = CHUNK_BYTES):
     """Every frame -> (coords (natoms, 3, F) float32 numpy [Angstrom], info as :func:`read_xyz_device`)."""
-    coords, info = _read(filename, _select(None), index, device, chunk_bytes)
+    coords, info = _read(filename, None, index, device, chunk_bytes)
     return coords.cpu().numpy(), info
 
 
 def read_xyz_frames(filename, frames, index: dict | None = None, device=None, chunk_bytes: int = CHUNK_BYTES):
     """:func:`read_xyz` for the listed frames (any order, repeats allowed; out of range raises IndexError)."""
-    coords, info = _read(filename, _select(frames), index, device, chunk_bytes)
+    coords, info = _read(filename, frames, index, device, chunk_bytes)
     return coords.cpu().numpy(), info
 
 
@@ -393,8 +348,6 @@ def _writer_args(coords, element, comment, chunk_bytes):
     natoms, _, F = (int(v) for v in coords.shape)
     if not 1 <= natoms <= MAX_ATOMS:
         raise ValueError(f"an XYZ frame written here holds 1 to {MAX_ATOMS} atoms, got {natoms}")
-    if isinstance(coords, torch.Tensor) and coords.dtype != torch.float32:
-        raise ValueError(f"coords must be float32, got {coords.dtype}")
     if isinstance(element, str) or len(element) != natoms:
         raise ValueError(f"element must be a sequence of {natoms} strings (one per atom)")
     for a, e in enumerate(element):
@@ -435,19 +388,12 @@ def _check_range(a) -> None:
 
 def _prepare(coords, element, comment, device, chunk_bytes):
     """every check, then (coords as a CUDA tensor or None without frames, natoms, F, head, column)"""
-    if isinstance(coords, torch.Tensor):
-        dev = _lib.tensor_device(coords, "write_xyz")
-    else:
-        coords = np.asarray(coords, dtype=np.float32)
-        dev = None
+    coords = _trajio.writer_coords(coords, "write_xyz")
     natoms, F, head, column = _writer_args(coords, element, comment, chunk_bytes)
     _check_range(coords)
     if F == 0:
         return None, natoms, F, head, column
-    if dev is None:
-        dev = _lib.device(device)
-        coords = torch.from_numpy(np.ascontiguousarray(coords)).to(dev)
-    return coords, natoms, F, head, column
+    return _trajio.on_device(coords, device), natoms, F, head, column
 
 
 def frame_bytes(natoms: int, head: bytes, width: int) -> int:

@@ -218,10 +218,9 @@ def test_arguments_are_checked_before_the_device_is_touched(tmp_path):
         with pytest.raises(ValueError):
             pd.dcd_bytes(*args, **kw)
         fn = tmp_path / "untouched.dcd"
-        if "chunk_bytes" not in kw:
-            with pytest.raises(ValueError):
-                pd.write_dcd(str(fn), *args, **kw)
-            assert not fn.exists()
+        with pytest.raises(ValueError):
+            pd.write_dcd(str(fn), *args, **kw)
+        assert not fn.exists()
     with pytest.raises(_lib.MkbError, match="no CPU fallback"):
         pd.encode_dcd_device(torch.zeros((12, 3, 4)))
     with pytest.raises(_lib.MkbError, match="no CPU fallback"):

@@ -221,24 +221,6 @@ def test_header_and_record_bytes_match_scipy(title, with_box):
     assert idx["n_frames"] == 0 and idx["natoms"] == N
 
 
-def test_slab_gather_reads_only_the_slabs(tmp_path):
-    from moleculekit_b200 import netcdf as pn
-
-    rng = np.random.default_rng(4)
-    raw = rng.integers(0, 256, size=300000, dtype=np.uint8)
-    fn = tmp_path / "bytes"
-    fn.write_bytes(raw.tobytes())
-    slab = 96
-    for starts in (np.arange(0, 200000, 100), np.arange(0, 290000, 96), np.array([8, 104, 5000, 5096, 299900 - 96]),
-                   np.sort(rng.choice(2000, size=700, replace=False)) * 140 + 4, np.arange(0, 1100 * 200, 200)):
-        out = np.zeros((len(starts), slab), np.uint8)
-        with open(fn, "rb") as fh:
-            pn._gather_slabs(fh.fileno(), starts.astype(np.int64), slab, out)
-        assert np.array_equal(out, raw[starts[:, None] + np.arange(slab)[None, :]])
-    with open(fn, "rb") as fh, pytest.raises(RuntimeError, match="changed while it was read"):
-        pn._gather_slabs(fh.fileno(), np.array([299990], np.int64), slab, np.zeros((1, slab), np.uint8))
-
-
 def test_arguments_are_checked_before_the_device_is_touched(tmp_path):
     import torch
     from moleculekit_b200 import _lib
