@@ -55,7 +55,7 @@ __device__ __forceinline__ bool bonded(const float *__restrict__ c, const float 
     if (is_h[i] && is_h[j]) return false;
     const float dx = __fsub_rn(c[3 * i], c[3 * j]), dy = __fsub_rn(c[3 * i + 1], c[3 * j + 1]),
                 dz = __fsub_rn(c[3 * i + 2], c[3 * j + 2]);
-    const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+    const float d2 = sq3(dx, dy, dz);
     if (d2 > cutoff2 || (double)d2 < 0.001) return false;
     const float cut = (float)(0.6 * (double)__fadd_rn(radii[i], radii[j]));
     return !(d2 > __fmul_rn(cut, cut));
@@ -230,7 +230,7 @@ __global__ void within_kernel(const float *__restrict__ coords, const unsigned *
             const float *s = src + 3ll * order[t];
             // atoms of other cells sharing the bucket are simply tested as well: any true hit is a valid answer
             const float dx = __fsub_rn(x, s[0]), dy = __fsub_rn(y, s[1]), dz = __fsub_rn(z, s[2]);
-            const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+            const float d2 = sq3(dx, dy, dz);
             if (d2 < sq_cutoff) { results[ii] = 1; return; }
         }
     }

@@ -240,4 +240,10 @@ __device__ __forceinline__ void fit_transform(const double (&R)[9], const double
         y[d] = __double2float_rn(fma(R[3 * d + 2], x2, fma(R[3 * d + 1], x1, R[3 * d] * x0)) + qb[d]);
 }
 
+// fl(fl(fl(dx dx) + fl(dy dy)) + fl(dz dz)): the reference's float32 squared norm, the one definition every pair kernel
+// compares and sums with
+__device__ __forceinline__ float sq3(float dx, float dy, float dz) {
+    return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+}
+
 }  // namespace mkb

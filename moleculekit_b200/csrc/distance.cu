@@ -22,54 +22,9 @@
 #include <cstring>
 
 #include "common.cuh"
+#include "pairs.cuh"
 
 namespace mkb {
-
-// d - b * roundf(d / b) with every op rounded to float (distance_utils.pyx:50-52).
-// Fast path: q~ = d * (1/b) differs from fl(d/b) by <= 2 ulp, and round-to-nearest-integer of q~ (magic-number add)
-// equals roundf(fl(d/b)) unless a half-integer lies within that error; those cases (and huge / non-finite quotients)
-// take the exact division + roundf.
-__device__ __forceinline__ float wrap_axis(float d, float b, float rb) {
-    const float q = __fmul_rn(d, rb);
-    float n = __fsub_rn(__fadd_rn(q, 12582912.0f), 12582912.0f);
-    const float fr = fabsf(__fsub_rn(q, n));
-    const float lim = fmaf(-6e-7f, fabsf(q), 0.5f);  // negative for |q| > 8e5 -> always exact path; NaN -> exact path
-    if (!(fr < lim)) n = roundf(__fdiv_rn(d, b));
-    return __fsub_rn(d, __fmul_rn(b, n));
-}
-
-__device__ __forceinline__ float sq3(float dx, float dy, float dz) {
-    return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-}
-
-struct BoxF {
-    float bx, by, bz, rx, ry, rz;
-    float hx, hy, hz;  // b / 2
-};
-
-__device__ __forceinline__ BoxF load_box(const float *box, long long stride, long long f) {
-    BoxF b;
-    b.bx = box[f];
-    b.by = box[stride + f];
-    b.bz = box[2 * stride + f];
-    b.rx = __frcp_rn(b.bx);
-    b.ry = __frcp_rn(b.by);
-    b.rz = __frcp_rn(b.bz);
-    b.hx = __fmul_rn(b.bx, 0.5f); b.hy = __fmul_rn(b.by, 0.5f); b.hz = __fmul_rn(b.bz, 0.5f);
-    asm volatile("" : "+f"(b.hx), "+f"(b.hy), "+f"(b.hz));  // keep the halves in registers (else recomputed per pair)
-    return b;
-}
-
-// squared distance of two gathered atoms, distance_utils.pyx:34-54 (_dist) / :188-206 (_dist2)
-__device__ __forceinline__ float pair_d2(const float4 a, const float4 b, const BoxF &bx, bool wrap) {
-    float dx = __fsub_rn(a.x, b.x), dy = __fsub_rn(a.y, b.y), dz = __fsub_rn(a.z, b.z);
-    if (wrap) {
-        dx = wrap_axis(dx, bx.bx, bx.rx);
-        dy = wrap_axis(dy, bx.by, bx.ry);
-        dz = wrap_axis(dz, bx.bz, bx.rz);
-    }
-    return sq3(dx, dy, dz);
-}
 
 // store with the fused host post-ops of projections/util.py:74-84: results[results > truncate] = truncate, then
 // (contacts) results <= threshold.  NaN distances stay NaN / compare false exactly like numpy.
@@ -82,33 +37,11 @@ __device__ __forceinline__ void store_dist(void *out, long long idx, float d, fl
     else reinterpret_cast<float *>(out)[idx] = d;
 }
 
-// ---------------------------------------------------------------------------------------------------------
-// gather + transpose: G[f][k] = (coords[idx[k], 0..2, f], chain bits) ; 32 frames x 32 atoms per CTA
-// ---------------------------------------------------------------------------------------------------------
-template <typename IdxT>
-__global__ void gather_kernel(const float *__restrict__ coords, long long stride, long long n_frames,
-                              const IdxT *__restrict__ idx, long long n, const unsigned *__restrict__ tag,
-                              float4 *__restrict__ G) {
-    __shared__ float tile[3][32][33];
-    const long long f0 = (long long)blockIdx.x * 32, k0 = (long long)blockIdx.y * 32;
-    const int lane = threadIdx.x, row = threadIdx.y;  // blockDim = (32, 8)
-    for (int kk = row; kk < 32; kk += 8) {
-        const long long k = k0 + kk, f = f0 + lane;
-        if (k < n && f < n_frames) {
-            const long long a = (long long)idx[k];
-#pragma unroll
-            for (int d = 0; d < 3; ++d) tile[d][kk][lane] = coords[(a * 3 + d) * stride + f];
-        }
-    }
-    __syncthreads();
-    for (int ff = row; ff < 32; ff += 8) {
-        const long long f = f0 + ff, k = k0 + lane;
-        if (k < n && f < n_frames) {
-            const unsigned t = tag ? tag[(long long)idx[k]] : 0u;
-            G[f * n + k] = make_float4(tile[0][lane][ff], tile[1][lane][ff], tile[2][lane][ff], __uint_as_float(t));
-        }
-    }
-}
+// the chain-id word of every gathered atom, or 0 without one (K5)
+struct AtomTag {
+    const unsigned *tag;
+    __device__ unsigned operator()(long long a) const { return tag ? tag[a] : 0u; }
+};
 
 template <typename IdxT>
 static int launch_gather(mkb_ctx *h, cudaStream_t st, const mkb_traj *t, const IdxT *idx, int64_t n,
@@ -116,7 +49,7 @@ static int launch_gather(mkb_ctx *h, cudaStream_t st, const mkb_traj *t, const I
     if (n == 0 || t->n_frames == 0) return MKB_OK;
     dim3 grid((unsigned)cdiv(t->n_frames, 32), (unsigned)cdiv(n, 32));
     if (grid.y > 65535) return fail(h, MKB_ERR_BAD_ARG, "selection too large (%lld atoms)", (long long)n);
-    gather_kernel<IdxT><<<grid, dim3(32, 8), 0, st>>>(t->coords, t->frame_stride, t->n_frames, idx, n, tag, G);
+    gather_kernel<IdxT, AtomTag><<<grid, dim3(32, 8), 0, st>>>(t->coords, t->frame_stride, t->n_frames, idx, n, AtomTag{tag}, G);
     MKB_LAUNCHED(h);
     return MKB_OK;
 }
@@ -127,43 +60,9 @@ static int launch_gather(mkb_ctx *h, cudaStream_t st, const mkb_traj *t, const I
 constexpr int K3_ROWS = 16;
 constexpr int K3_COLS = 256;
 
-// Minimum-image step of the dense kernels: n = rint(d * fl(1/b)) by the magic-number trick, w = d - fl(b n) exactly as
-// the reference rounds it (pyx:41-49), and ONE test that n is the reference's roundf(fl(d / b)):  |w| < b/2 - 1e-6 |d|.
-// If the two integers differed, d/b would lie within 2e-7 |d/b| of a half-integer, hence |w| >= b/2 - 3e-7 |d| and the
-// test fails; exact ties (|w| == b/2: half-away vs half-even), |d/b| >= 2^22 (magic rounding invalid), NaN and boxes
-// that are zero / negative / non-finite fail it as well.  One rare branch per PAIR then redoes the flagged pair with the
-// general wrap_axis (exact division).  7 instructions per axis instead of 9 for the former quotient-distance test.
-__device__ __forceinline__ float wrap_fast(float d, float b, float rb, float hb, bool &risky) {
-    const float q = __fmul_rn(d, rb);
-    const float n = __fsub_rn(__fadd_rn(q, 12582912.0f), 12582912.0f);
-    const float w = __fsub_rn(d, __fmul_rn(b, n));
-    risky = risky | !(fabsf(w) < fmaf(-1e-6f, fabsf(d), hb));
-    return w;
-}
-
-__device__ __forceinline__ float pair_d2_fastwrap(const float4 a, const float4 b, unsigned cb, const BoxF &bx, int pbc) {
-    float dx = __fsub_rn(a.x, b.x), dy = __fsub_rn(a.y, b.y), dz = __fsub_rn(a.z, b.z);
-    if (pbc && (__float_as_uint(a.w) != cb)) {
-        bool risky = false;
-        const float wx = wrap_fast(dx, bx.bx, bx.rx, bx.hx, risky), wy = wrap_fast(dy, bx.by, bx.ry, bx.hy, risky),
-                    wz = wrap_fast(dz, bx.bz, bx.rz, bx.hz, risky);
-        if (risky) {
-            dx = wrap_axis(dx, bx.bx, bx.rx);
-            dy = wrap_axis(dy, bx.by, bx.ry);
-            dz = wrap_axis(dz, bx.bz, bx.rz);
-        } else {
-            dx = wx; dy = wy; dz = wz;
-        }
-    }
-    return sq3(dx, dy, dz);
-}
-
-// K3 hot loop variant: the rare exact re-wrap is an out-of-line call (the inlined form merged its registers back with a
-// dozen MOV / BSSY / BSYNC per pair), the half boxes live in registers, and the threshold folds |d| in with one FFMA:
+// K3 hot loop variant: the rare exact re-wrap is an out-of-line call (pair_d2_rewrap), the half boxes live in registers,
+// and the threshold folds |d| in with one FFMA:
 //   risky  <=>  |w| + 1e-6 |d| >= b/2  on some axis   (the same test as wrap_fast, rearranged)
-__device__ __noinline__ float pair_d2_rewrap(float dx, float dy, float dz, float bxx, float bxy, float bxz, float rx, float ry, float rz) {
-    return sq3(wrap_axis(dx, bxx, rx), wrap_axis(dy, bxy, ry), wrap_axis(dz, bxz, rz));
-}
 __device__ __forceinline__ float pair_d2_lean(const float4 a, const float4 b, unsigned cb, const BoxF &bx, int pbc) {
     const float dx = __fsub_rn(a.x, b.x), dy = __fsub_rn(a.y, b.y), dz = __fsub_rn(a.z, b.z);
     if (!(pbc && (__float_as_uint(a.w) != cb))) return sq3(dx, dy, dz);
@@ -175,24 +74,6 @@ __device__ __forceinline__ float pair_d2_lean(const float4 a, const float4 b, un
                       (fmaf(1e-6f, fabsf(dz), fabsf(wz)) < bx.hz);
     if (!safe) return pair_d2_rewrap(dx, dy, dz, bx.bx, bx.by, bx.bz, bx.rx, bx.ry, bx.rz);
     return sq3(wx, wy, wz);
-}
-
-// same with the wrap decision made by the caller (group chains, K5)
-__device__ __forceinline__ float pair_d2_fastwrap_flag(const float4 a, const float4 b, const BoxF &bx, bool wrap) {
-    float dx = __fsub_rn(a.x, b.x), dy = __fsub_rn(a.y, b.y), dz = __fsub_rn(a.z, b.z);
-    if (wrap) {
-        bool risky = false;
-        const float wx = wrap_fast(dx, bx.bx, bx.rx, bx.hx, risky), wy = wrap_fast(dy, bx.by, bx.ry, bx.hy, risky),
-                    wz = wrap_fast(dz, bx.bz, bx.rz, bx.hz, risky);
-        if (risky) {
-            dx = wrap_axis(dx, bx.bx, bx.rx);
-            dy = wrap_axis(dy, bx.by, bx.ry);
-            dz = wrap_axis(dz, bx.bz, bx.rz);
-        } else {
-            dx = wx; dy = wy; dz = wz;
-        }
-    }
-    return sq3(dx, dy, dz);
 }
 
 // Contact maps only need the BOOLEAN d2 <= T of the reference's float32 sequence, not its bits.  A fused estimate of d2

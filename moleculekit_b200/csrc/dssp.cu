@@ -150,7 +150,7 @@ __global__ void __launch_bounds__(DS_THREADS) dssp_hbond_kernel(const DsArgs A, 
             if (a == d || a == d - 1) continue;
             const float4 ca = S.ca[base + a];
             const float dx = __fsub_rn(ca.x, cd.x), dy = __fsub_rn(ca.y, cd.y), dz = __fsub_rn(ca.z, cd.z);
-            const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+            const float d2 = sq3(dx, dy, dz);
             if (d2 > 82.f) continue;  // the float64 distance is > 9 there
             if (ds_dist(cd.x, cd.y, cd.z, ca.x, ca.y, ca.z) < 9.0) {
                 const double e = ds_energy(D, S.rec[base + a]);

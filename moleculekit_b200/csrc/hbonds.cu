@@ -18,63 +18,30 @@
 // 10 million; tests/test_oracle_golden.py::test_hbonds_float_overloads).  Every operation has an IEEE counterpart on the
 // device (__f*_rn, __ddiv_rn) except acosf.  acosf is a non-increasing function of its float argument, so the host finds,
 // with the same libm the reference calls, the largest float c* whose arc cosine still exceeds the threshold; the device
-// tests c <= c* -- the same booleans without a device acos (the trick K3 uses for sqrt).
+// tests c <= c* -- the same booleans without a device acos (the trick K3 uses for sqrt).  The wrap is pairs.cuh's
+// minimum-image step under the interactions rule (wrap_fast_if, with wrap_axis_if for flagged pairs).
 #include <cmath>
 #include <cstring>
 
 #include <cub/device/device_scan.cuh>
 
 #include "common.cuh"
+#include "pairs.cuh"
 
 namespace mkb {
 
-// G[f][k] = (coords[idx[k], 0..2, f], tag of idx[k]); tag bit0: sel1 != 0, bit1: sel1 == 1, bit2: sel2 == 1, bits 3..31: the
-// atom index itself (n_atoms < 2^29), so the pair loop needs no second load
-__global__ void hb_gather_kernel(const float *__restrict__ coords, long long stride, long long n_frames,
-                                 const unsigned *__restrict__ idx, long long n, const unsigned *__restrict__ sel1,
-                                 const unsigned *__restrict__ sel2, float4 *__restrict__ G) {
-    __shared__ float tile[3][32][33];
-    const long long f0 = (long long)blockIdx.x * 32, k0 = (long long)blockIdx.y * 32;
-    const int lane = threadIdx.x, row = threadIdx.y;  // blockDim = (32, 8)
-    for (int kk = row; kk < 32; kk += 8) {
-        const long long k = k0 + kk, f = f0 + lane;
-        if (k < n && f < n_frames) {
-            const long long a = (long long)idx[k];
-#pragma unroll
-            for (int d = 0; d < 3; ++d) tile[d][kk][lane] = coords[(a * 3 + d) * stride + f];
-        }
+// the record word of a gathered donor / acceptor: bit0: sel1 != 0, bit1: sel1 == 1, bit2: sel2 == 1, bits 3..31: the atom
+// index itself (n_atoms < 2^29), so the pair loop needs no second load
+struct HbTag {
+    const unsigned *sel1, *sel2;
+    __device__ unsigned operator()(long long a) const {
+        const unsigned s1 = sel1[a], s2 = sel2[a];
+        return (s1 != 0u ? 1u : 0u) | (s1 == 1u ? 2u : 0u) | (s2 == 1u ? 4u : 0u) | ((unsigned)a << 3);
     }
-    __syncthreads();
-    for (int ff = row; ff < 32; ff += 8) {
-        const long long f = f0 + ff, k = k0 + lane;
-        if (k < n && f < n_frames) {
-            const long long a = (long long)idx[k];
-            const unsigned s1 = sel1[a], s2 = sel2[a];
-            const unsigned t = (s1 != 0u ? 1u : 0u) | (s1 == 1u ? 2u : 0u) | (s2 == 1u ? 4u : 0u) | ((unsigned)a << 3);
-            G[f * n + k] = make_float4(tile[0][lane][ff], tile[1][lane][ff], tile[2][lane][ff], __uint_as_float(t));
-        }
-    }
-}
+};
 
-// pyx:88-94: one component of a minimum-image vector, every operation rounded to float (general path)
-__device__ __noinline__ float hb_wrap_exact(float val, float b, float hb) {
-    if (fabsf(val) > hb && b != 0.f) val = __fsub_rn(val, __fmul_rn(b, roundf(__fdiv_rn(val, b))));
-    return val;
-}
-
-// Branch-free form of the same step for the pair loop: K3's wrap_fast (csrc/distance.cu).  n = rint(val * fl(1/b)) by the
-// magic-number trick, r = val - fl(b n) as the reference rounds it, and ONE test that n is the reference's
-// roundf(fl(val / b)):  |r| < b/2 - 1e-6 |val|.  Were the integers different, val / b would lie within 2e-7 of a half-integer
-// and |r| >= b/2 - 3e-7 |val|.  Exact ties, |val / b| >= 2^22, NaN and non-positive boxes fail the test; such pairs set
-// `risky` and are redone with hb_wrap_exact.  No wrap (|val| <= b/2 or b == 0) leaves val untouched, as there.
-__device__ __forceinline__ float hb_wrap_fast(float val, float b, float rb, float hb, bool &risky) {
-    const bool w = fabsf(val) > hb && b != 0.f;
-    const float MAGIC = 12582912.f;  // 1.5 * 2^23
-    const float n = __fsub_rn(__fadd_rn(__fmul_rn(val, rb), MAGIC), MAGIC);
-    const float r = __fsub_rn(val, __fmul_rn(b, n));
-    risky = risky || (w && !(fabsf(r) < __fmaf_rn(-1e-6f, fabsf(val), hb)));
-    return w ? r : val;
-}
+// pyx:88-94, kept out of line: the exact step is the rare path of the pair loop
+__device__ __noinline__ float hb_rewrap(float val, float b, float hb) { return wrap_axis_if(val, b, hb); }
 
 struct HbArgs {
     const float4 *GA;        // [F][na] acceptors
@@ -98,6 +65,7 @@ __global__ void __launch_bounds__(256) hbond_kernel(const HbArgs A, long long *_
     const float4 ph = A.GD[row * 2], pH = A.GD[row * 2 + 1];
     const unsigned d_heavy = A.donors[2 * d], d_hyd = A.donors[2 * d + 1];
     const unsigned dbits = __float_as_uint(ph.w);
+    // read by hand rather than through load_box, which made this kernel about 1 % slower on an H100 (C10)
     const float bx = A.box[f], by = A.box[A.fsb + f], bz = A.box[2 * A.fsb + f];
     const float hx = __fdiv_rn(bx, 2.f), hy = __fdiv_rn(by, 2.f), hz = __fdiv_rn(bz, 2.f);
     const float rbx = __frcp_rn(bx), rby = __frcp_rn(by), rbz = __frcp_rn(bz);
@@ -105,10 +73,10 @@ __global__ void __launch_bounds__(256) hbond_kernel(const HbArgs A, long long *_
     // heavy -> hydrogen vector: the same for every acceptor of the row (pyx:107-114)
     float b0 = 0.f, b1 = 0.f, b2 = 0.f, d2b = 0.f;
     if (!A.ignore_hs) {
-        b0 = hb_wrap_exact(__fsub_rn(ph.x, pH.x), bx, hx);
-        b1 = hb_wrap_exact(__fsub_rn(ph.y, pH.y), by, hy);
-        b2 = hb_wrap_exact(__fsub_rn(ph.z, pH.z), bz, hz);
-        d2b = __fadd_rn(__fadd_rn(__fmul_rn(b0, b0), __fmul_rn(b1, b1)), __fmul_rn(b2, b2));
+        b0 = hb_rewrap(__fsub_rn(ph.x, pH.x), bx, hx);
+        b1 = hb_rewrap(__fsub_rn(ph.y, pH.y), by, hy);
+        b2 = hb_rewrap(__fsub_rn(ph.z, pH.z), bz, hz);
+        d2b = sq3(b0, b1, b2);
     }
     long long base = FILL ? row_offsets[row] : 0;
     const long long row_end = FILL ? row_offsets[row + 1] : 0;
@@ -130,13 +98,13 @@ __global__ void __launch_bounds__(256) hbond_kernel(const HbArgs A, long long *_
             if (ok) {
                 const float v0 = __fsub_rn(pa.x, pd.x), v1 = __fsub_rn(pa.y, pd.y), v2 = __fsub_rn(pa.z, pd.z);
                 bool risky = false;
-                float a0v = hb_wrap_fast(v0, bx, rbx, hx, risky);
-                float a1v = hb_wrap_fast(v1, by, rby, hy, risky);
-                float a2v = hb_wrap_fast(v2, bz, rbz, hz, risky);
+                float a0v = wrap_fast_if(v0, bx, rbx, hx, risky);
+                float a1v = wrap_fast_if(v1, by, rby, hy, risky);
+                float a2v = wrap_fast_if(v2, bz, rbz, hz, risky);
                 if (risky) {  // quotient next to a half-integer, or huge: the exactly rounded division
-                    a0v = hb_wrap_exact(v0, bx, hx); a1v = hb_wrap_exact(v1, by, hy); a2v = hb_wrap_exact(v2, bz, hz);
+                    a0v = hb_rewrap(v0, bx, hx); a1v = hb_rewrap(v1, by, hy); a2v = hb_rewrap(v2, bz, hz);
                 }
-                const float d2a = __fadd_rn(__fadd_rn(__fmul_rn(a0v, a0v), __fmul_rn(a1v, a1v)), __fmul_rn(a2v, a2v));
+                const float d2a = sq3(a0v, a1v, a2v);
                 if (!(d2a > A.thr2)) {                                             // pyx:97-98 (NaN passes, as there)
                     if (A.ignore_hs) {
                         hit = true;                                                // pyx:101-105
@@ -227,11 +195,12 @@ static int hb_setup(mkb_ctx *h, cudaStream_t st, const mkb_traj *t, const uint32
     const unsigned gx = (unsigned)cdiv(F, 32);
     const long long gya = cdiv(n_acceptors, 32), gyd = cdiv(2 * n_donors, 32);
     if (gya > 65535 || gyd > 65535) return fail(h, MKB_ERR_BAD_ARG, "too many donors / acceptors for one call");
-    hb_gather_kernel<<<dim3(gx, (unsigned)gya), dim3(32, 8), 0, st>>>(t->coords, t->frame_stride, F, acceptors, n_acceptors,
-                                                                      sel1, sel2, G);
+    gather_kernel<unsigned, HbTag><<<dim3(gx, (unsigned)gya), dim3(32, 8), 0, st>>>(t->coords, t->frame_stride, F, acceptors,
+                                                                                    n_acceptors, HbTag{sel1, sel2}, G);
     MKB_LAUNCHED(h);
-    hb_gather_kernel<<<dim3(gx, (unsigned)gyd), dim3(32, 8), 0, st>>>(t->coords, t->frame_stride, F, donors, 2 * n_donors,
-                                                                      sel1, sel2, G + F * n_acceptors);
+    gather_kernel<unsigned, HbTag><<<dim3(gx, (unsigned)gyd), dim3(32, 8), 0, st>>>(t->coords, t->frame_stride, F, donors,
+                                                                                    2 * n_donors, HbTag{sel1, sel2},
+                                                                                    G + F * n_acceptors);
     MKB_LAUNCHED(h);
     return MKB_OK;
 }

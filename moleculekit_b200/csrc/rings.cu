@@ -12,7 +12,8 @@
 //
 // Bit parity.  The modules are C++: round / sqrt / acos on float arguments are the float overloads (see hbonds.cu).  All
 // geometry is float with one rounding per operation (centroid = float sum in atom order / (float)count; wrapped distance
-// val - fl(box * roundf(fl(val / box))); cross product, norms by sqrtf): bit-identical on the device.  The decisions
+// val - fl(box * roundf(fl(val / box))), pairs.cuh's wrap_axis_if; cross product, norms by sqrtf): bit-identical on the
+// device.  The decisions
 // compare the DOUBLE `angle = fold((double)acosf(dot) * 57.29578)` with the thresholds; fold and every comparison are
 // monotone on each side of the fold, so the host turns each decision into at most two closed intervals of the float `dot`
 // (bisection with the libm the reference calls) and the device tests interval membership: the reference's booleans
@@ -24,6 +25,7 @@
 #include <cub/device/device_scan.cuh>
 
 #include "common.cuh"
+#include "pairs.cuh"
 
 namespace mkb {
 
@@ -52,17 +54,13 @@ __device__ __forceinline__ bool ring_in(const RingSet &s, float x) {
 // pyx:46-62 `_wrapped_dist`: every operation rounded to float
 __device__ __forceinline__ float ring_wdist(const float4 a, const float4 b, float bx, float by, float bz, float hx, float hy,
                                             float hz) {
-    float v0 = __fsub_rn(a.x, b.x), v1 = __fsub_rn(a.y, b.y), v2 = __fsub_rn(a.z, b.z);
-    if (fabsf(v0) > hx && bx != 0.f) v0 = __fsub_rn(v0, __fmul_rn(bx, roundf(__fdiv_rn(v0, bx))));
-    if (fabsf(v1) > hy && by != 0.f) v1 = __fsub_rn(v1, __fmul_rn(by, roundf(__fdiv_rn(v1, by))));
-    if (fabsf(v2) > hz && bz != 0.f) v2 = __fsub_rn(v2, __fmul_rn(bz, roundf(__fdiv_rn(v2, bz))));
-    return __fadd_rn(__fadd_rn(__fadd_rn(0.f, __fmul_rn(v0, v0)), __fmul_rn(v1, v1)), __fmul_rn(v2, v2));
+    const float v0 = __fsub_rn(a.x, b.x), v1 = __fsub_rn(a.y, b.y), v2 = __fsub_rn(a.z, b.z);
+    return sq3(wrap_axis_if(v0, bx, hx), wrap_axis_if(v1, by, hy), wrap_axis_if(v2, bz, hz));
 }
 
 // pyx:67-83: vec / sqrtf(sum of squares), float
 __device__ __forceinline__ void ring_normalize(float &x, float &y, float &z) {
-    float n = __fadd_rn(__fadd_rn(__fadd_rn(0.f, __fmul_rn(x, x)), __fmul_rn(y, y)), __fmul_rn(z, z));
-    n = __fsqrt_rn(n);
+    const float n = __fsqrt_rn(sq3(x, y, z));
     x = __fdiv_rn(x, n); y = __fdiv_rn(y, n); z = __fdiv_rn(z, n);
 }
 

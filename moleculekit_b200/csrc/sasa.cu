@@ -78,8 +78,7 @@ __device__ __forceinline__ int sa_hash(long long cx, long long cy, long long cz,
 
 // fl(fl(fl(a.x b.x) + fl(a.y b.y)) + fl(a.z b.z)) of the difference a - b: SSE dpps with mask 0x71
 __device__ __forceinline__ float sa_d2(float ax, float ay, float az, float bx, float by, float bz) {
-    const float dx = __fsub_rn(ax, bx), dy = __fsub_rn(ay, by), dz = __fsub_rn(az, bz);
-    return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+    return sq3(__fsub_rn(ax, bx), __fsub_rn(ay, by), __fsub_rn(az, bz));
 }
 
 __global__ void sasa_maxr_kernel(const float *__restrict__ radii, long long n, float *__restrict__ maxr) {
