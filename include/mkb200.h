@@ -706,6 +706,76 @@ int mkb_tmscore(mkb_handle_t h, void *stream, const mkb_traj *t, const uint32_t 
                 double *rmsd);
 int64_t mkb_tmscore_max_pairs(void);
 
+/* K27: TM-align, replaces the TM-align program (Zhang & Skolnick, Nucleic Acids Res. 2005) that moleculekit's
+ * molTMalign runs per frame: a sequence-independent residue alignment and superposition of x, the mol CA trace (atom
+ * rows sel[0..xlen) of t), onto y, the reference trace (atom rows refsel[0..ylen) of ref).  All pointers except the
+ * mkb_traj structs and params are device pointers.  5 <= xlen, ylen <= mkb_tmalign_max_residues() (TM-align's "too
+ * short" below 5).  ref_per_frame = 0: every item against frame 0 of ref; 1: item k against frame f of ref, f its own
+ * listed frame (ref n_frames >= t n_frames).  frames [n_frames] uint32 = the listed frames of t (NULL = every frame).
+ * Index ranges are the caller's responsibility.  The restatement is tests/tmalign_oracle.c, in the shape of the C++
+ * release's TMalign_main; invmap[j] is the x residue aligned to y residue j, or -1; dist is the SQUARED distance.
+ *
+ * params [10] host float64 (tmalign_parameters, C pow): Lnorm = min(xlen, ylen); d0 = 0.168 if Lnorm <= 19 else
+ * 1.24 (Lnorm - 15)^(1/3) - 1.8; D0_MIN = d0 + 0.8 and d0 = D0_MIN; d0_search = d0 clamped to [4.5, 8]; score_d8 =
+ * 1.5 Lnorm^0.3 + 3.5; ddcc = 0.1 if Lnorm <= 40 else 0.4; dcu0 = 4.25: [d0, d0_search, score_d8, D0_MIN, ddcc,
+ * dcu0], then the final d0 (0.5 if L <= 21 else the same formula, floored at 0.5) and its clamped d0_search for
+ * L = ylen, then for L = xlen.
+ *
+ * Per item, everything in float64 from the float32 coordinates, every operation rounded on its own (no fused
+ * multiply-add), every sum sequential in pair order:
+ *   fit       K19's: two-pass centroids p, q and H, Horn's quaternion by cyclic Jacobi; x' = R (x - p) + q, each row
+ *             ((R0 a0 + R1 a1) + R2 a2) + q with a = x - p; dist = (dx dx + dy dy) + dz dz.  An empty set fits the
+ *             identity.
+ *   sec       residue i with i - 2, i + 2 in range: the square roots d13 d14 d15 d24 d25 d35 over i - 2 .. i + 2; H when
+ *             |d15 - 6.37|, |d14 - 5.18|, |d25 - 5.18|, |d13 - 5.45|, |d24 - 5.45|, |d35 - 5.45| are all < 2.1, else E
+ *             against 13, 10.4, 10.4, 6.1, 6.1, 6.1 and 1.42, else T when d15 < 8, else C (also without neighbours).
+ *   score_fun8  cut at dist < (d + inc 0.5)^2, inc = 0, 1, ... while fewer than 3 pairs and n > 3; method 8 sums
+ *             1 / (1 + dist / d0^2) over pairs with dist <= score_d8^2, method 0 over all; divided by Lnorm (the
+ *             standard form: by n).
+ *   TMscore8_search  over n pairs: fragment lengths n >> i while > min(4, n), then min(4, n) (at most 6); starts 0,
+ *             +simplify_step, the last start n - L always; each start: seed fit, cut at d0_search - 1, then up to 20
+ *             refits of the cut set cut at d0_search + 1, stopping on an empty set or a repeated one; the best score
+ *             (strict >) and its fit.  An empty pair set scores 0 with the identity.
+ *   get_score_fast  fit all pairs of the map, score; refit dist <= d0_search^2 (+0.5 while < 3 pairs and n > 3) and,
+ *             when that set is not all pairs, once more at d0_search^2 + 1; the largest of the three (>=).
+ *   NWDP_TM   value d = val[i-1][j-1] + term (1 / (1 + dist / d02) under a fit; that + 0.5 where the codes match;
+ *             1 where they match), h / v = the neighbour + gap_open when that neighbour took its diagonal; the
+ *             diagonal when d >= h && d >= v, else v when v >= h, else h; traceback from (xlen, ylen) by the same rule.
+ *   DP_iter   for gap_open in {-0.6, 0}[g1..g2), up to the iteration count: DP under the current fit with d02 = d0^2,
+ *             detailed_search (simplify_step 40, method 8) whose fit is the next one; keep the best map (>); stop when
+ *             |TM_old - TM| < 1e-6 (TM_old is carried across the gap opens).
+ *   initial   1 gapless threading over every shift, min_ali = max(5, min_len / 2), best shift on >=; DP_iter(0, 2, 30).
+ *             2 DP on the codes, gap -1; DP_iter(0, 2, 30) if TM > 0.2 TMmax.  3 get_initial5: fragment lengths {20,
+ *             100} capped at aL / 3, aL / 2, jumps 45 / 35 / 25 / 15 for lengths > 250 / > 200 / > 150 / else, capped
+ *             at len / 3; per fragment pair a fit, DP with gap 0 and d01 = max(d0 + 1.5, D0_MIN), get_score_fast, first
+ *             maximum (>) wins; DP_iter(0, 2, 2) if TM > ddcc TMmax.  4 the score 1 / (1 + dist / d01^2) (+ 0.5 where
+ *             the codes match) under the fit of the best map, gap -1; DP_iter(0, 2, 30) if TM > ddcc TMmax.  5
+ *             find_max_frag on both traces (cutoff dcu0 grown by a running product of 1.1 until the longest run of
+ *             consecutive dist < cutoff^2 has min(4, len / 3) residues), the x fragment when Lx < Ly or Lx == Ly and
+ *             xlen <= ylen, else the y one, trimmed to [floor(0.1 L0), floor(0.89 L0)] when it spans L0 =
+ *             min(xlen, ylen), threaded with min_ali = max(3, floor(min_len / 2.5)), best on >=; DP_iter(1, 2, 2) if
+ *             TM > ddcc TMmax.  Each initial map first goes through detailed_search (40, method 8); TMmax and the
+ *             best map update on strict >.
+ *   final     detailed_search_standard (simplify_step 1, method 8) on the best map; under its fit the aligned pairs
+ *             with sqrt(dist) <= score_d8 are the nali final pairs (invmap keeps only them); rmsd = sqrt(sum dist /
+ *             nali) under the fit of those pairs; tm[k][0] = TMscore8_search (simplify_step 1, method 0) over them
+ *             with the final parameters of L = ylen, whose best fit is records[k]; tm[k][1] the same for L = xlen.
+ *             nali = 0 gives scores and rmsd 0 and the identity record.
+ * Outputs per item k: tm [n][2], rmsd [n], nali [n] int32, invmap [n][ylen] int32, records [n][16] in K14's layout
+ * (R row-major, p, q, pad; mkb_align_apply moves frames with them).  A non-finite selected coordinate (of the frame or
+ * its reference frame) gives NaN scores and rmsd, nali 0, invmap all -1 and the identity record, in that item only.
+ * Not confirmed against TMalign.cpp (no source at hand): the fit (the program uses its own Kabsch routine), the
+ * running product in place of pow(1.1, inc), the 2019 release's extra tie search for Lx == Ly and xlen == ylen (left
+ * out), the final search's simplify_step, and that the alignment reported is the score_d8-filtered map.
+ * One warp per item; per-item state in global scratch, items in chunks of mkb_tmalign_chunk_frames(xlen, ylen).
+ * The handle's timing events bracket the launches (main; prep is empty). */
+int mkb_tmalign(mkb_handle_t h, void *stream, const mkb_traj *t, const uint32_t *sel, int64_t xlen, const mkb_traj *ref,
+                const uint32_t *refsel, int64_t ylen, int32_t ref_per_frame, const double *params,
+                const uint32_t *frames, int64_t n_frames, double *tm, double *rmsd, int32_t *nali, int32_t *invmap,
+                double *records);
+int64_t mkb_tmalign_max_residues(void);
+int64_t mkb_tmalign_chunk_frames(int64_t xlen, int64_t ylen);
+
 #ifdef __cplusplus
 }
 #endif

@@ -48,7 +48,7 @@ EXPORTS = [
     "mkb_wrap_triclinic", "mkb_hbonds_count", "mkb_hbonds_fill", "mkb_ring_pairs_count", "mkb_ring_pairs_fill",
     "mkb_align_fit", "mkb_align_apply", "mkb_rmsd", "mkb_coordinates", "mkb_coord_sums", "mkb_fluctuation",
     "mkb_frame_moments", "mkb_dihedrals", "mkb_sasa", "mkb_sasa_chunk_frames", "mkb_dssp", "mkb_dssp_chunk_frames",
-    "mkb_tmscore", "mkb_tmscore_max_pairs",
+    "mkb_tmscore", "mkb_tmscore_max_pairs", "mkb_tmalign", "mkb_tmalign_max_residues", "mkb_tmalign_chunk_frames",
 ]
 
 _lib = None
@@ -152,9 +152,15 @@ def load():
     lib.mkb_tmscore.argtypes = [vp, vp, tp, vp, tp, vp, i64, i64, C.c_double, C.c_double, vp, i32, vp, i64, vp, vp]
     lib.mkb_tmscore_max_pairs.argtypes = []
     lib.mkb_tmscore_max_pairs.restype = i64
+    lib.mkb_tmalign.argtypes = [vp, vp, tp, vp, i64, tp, vp, i64, i32, vp, vp, i64, vp, vp, vp, vp, vp]
+    lib.mkb_tmalign_max_residues.argtypes = []
+    lib.mkb_tmalign_max_residues.restype = i64
+    lib.mkb_tmalign_chunk_frames.argtypes = [i64, i64]
+    lib.mkb_tmalign_chunk_frames.restype = i64
     for name in EXPORTS:
         if name in ("mkb_last_error", "mkb_launch_count", "mkb_version", "mkb_last_kernel", "mkb_occupancy_compact_blocks",
-                    "mkb_sasa_chunk_frames", "mkb_dssp_chunk_frames", "mkb_tmscore_max_pairs"):
+                    "mkb_sasa_chunk_frames", "mkb_dssp_chunk_frames", "mkb_tmscore_max_pairs",
+                    "mkb_tmalign_max_residues", "mkb_tmalign_chunk_frames"):
             continue
         getattr(lib, name).restype = C.c_int
     _lib = lib

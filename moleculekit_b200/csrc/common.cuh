@@ -53,6 +53,7 @@ enum ScratchSlot {
     S_XYZ_STARTS,   // K26: line starts of the staged frames
     S_XYZ_STATE,    // K26: the decode's running line count
     S_BOND_MIN,     // K7: per-axis coordinate minimum (the reference's xyzmin) as order keys
+    S_TMALIGN,      // K27: per-item traces, index lists and DP state of one item chunk
     S_NSLOTS
 };
 
