@@ -438,6 +438,60 @@ int mkb_xyz_encode(mkb_handle_t h, void *stream, const float *coords, int64_t fr
                    int64_t natoms, const uint8_t *head, int64_t head_bytes, const uint8_t *elements, int64_t width,
                    uint8_t *out, int64_t out_capacity);
 
+/* K28: the index pass over a chunk of a multi-model PDB file; replaces the host reader's line loop as far as finding
+ * the frames.  The frame rules (the host applies them to the list this pass builds):
+ *   - an atom record is a line whose first six bytes are "ATOM  " or "HETATM"; every other record is skipped;
+ *   - with MODEL records (first five bytes "MODEL", then a space or the line's end) each MODEL starts a frame that runs
+ *     to the next MODEL, ENDMDL or END record (first three bytes "END", then a space or the line's end) or the end of
+ *     the file; without them the file is one frame of the atom records before the first ENDMDL / END;
+ *   - natoms is frame 0's atom record count and every other frame holds exactly natoms; a last model cut short by the
+ *     end of the file (no ENDMDL / END after it) is dropped;
+ *   - a frame's cell is the last CRYST1 record before its first atom record.
+ * bytes = the chunk on the device, 16-byte aligned: the file's bytes [file_base, file_base + n_read), of which the line
+ * starts after the newlines in the first n are classified (n_read - n bytes of look-ahead, at least 6, let the last
+ * lines be read); byte 0 starts a line when file_base == 0.  state (device int64[3], 8-byte aligned; the caller sets
+ * {0, INT64_MAX, 0} before the first chunk and keeps it across chunks, which run in file order on one stream): [0] the
+ * running atom record count, [1] the atomic minimum file offset of a CR not followed by LF, [2] the number of marks.
+ * Every MODEL, ENDMDL, END and CRYST1 record appends (file offset * 8 + kind, atom records before it in the file) to
+ * marks (device int64[2 * mark_cap]) at slot state[2]++ while the slot is below mark_cap; kind 2 MODEL, 3 ENDMDL, 4 END,
+ * 5 CRYST1.  The slots are in no particular order. */
+int mkb_pdb_index(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t n, int64_t n_read, int64_t file_base,
+                  int64_t *state, int64_t *marks, int64_t mark_cap);
+
+/* K28: PDB frames parsed on the device; replaces the host reader's float() of columns 31-38, 39-46 and 47-54 of every
+ * atom record and the host transposition to the frame-minor array.  bytes = n_staged whole frames back to back on the
+ * device, 16-byte aligned, nbytes long and readable up to nbytes rounded up to 16; each staged frame starts a line,
+ * holds exactly natoms atom records and (but for the last) ends in '\n'.  frame_of (HOST int32[n_frames]) = the staged
+ * frame of listed frame k.  coords (natoms, 3, n_frames) float32 device, element (a, d, k) at coords[(a*3 + d)*
+ * frame_stride + k] = field d of atom record a, bit for bit np.float32(float(field)): the F8.3 fast path, else the
+ * grammar of mkb_xyz_decode within the 8-byte field.  A line shorter than 54 columns (a '\n' or '\r' before column 55),
+ * an empty field, a field outside the grammar, a byte >= 0x80 or an undecided rounding is flagged: flags (device int64,
+ * 8-byte aligned, flags[0] set to 0 by the caller) receives (frame_base + k) * natoms + a at flags[1 + j] for j <
+ * flag_cap, and flags[0] counts every flagged line; such a line's coordinates are unspecified. */
+int mkb_pdb_decode(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t nbytes, int64_t n_staged,
+                   const int32_t *frame_of, int64_t n_frames, int64_t natoms, float *coords, int64_t frame_stride,
+                   int64_t frame_base, int64_t *flags, int64_t flag_cap);
+
+/* K28: CRYST1 records parsed on the device.  rows (device, 16-byte aligned) holds n_cells rows of 64 bytes, each the
+ * first 54 (or more) bytes of a CRYST1 line.  cells (device float32[6 * n_cells]) = a, b, c (columns 7-15, 16-24,
+ * 25-33) and alpha, beta, gamma (columns 34-40, 41-47, 48-54) of row i at cells[6 i + d], each bit for bit
+ * np.float32(float(field)); bad (device int32[n_cells]) = 1 where the row's fields are left to the host (as for
+ * mkb_pdb_decode's flags), else 0. */
+int mkb_pdb_cell(mkb_handle_t h, void *stream, const uint8_t *rows, int64_t n_cells, float *cells, int32_t *bad);
+
+/* K28: PDB frames written on the device, the inverse of mkb_pdb_decode.  coords float32 device, element (a, d, k) at
+ * coords[(a*3 + d)*frame_stride + k]; box and angles (3, n_frames) float32 device at [d*box_stride + k], or box NULL for
+ * frames without a CRYST1 line.  Frame k is written at out + k*S, S = 15 + (box ? 71 : 0) + 81*natoms + 7:
+ * "MODEL %8d\n" of model0 + k + 1, with a box "CRYST1%9.3f%9.3f%9.3f%7.2f%7.2f%7.2f P 1           1\n", then per atom
+ * the 81 bytes of tmpl[a*81 ...] (device, readable up to 81*natoms rounded up to 4) with '%8.3f' of x, y and z in
+ * columns 31-54, then "ENDMDL\n".  Each field is byte for byte Python's '%W.Df': rint(x * 10^D) in float64 (exact,
+ * half to even), the sign printed whenever x is negative or -0.0; the caller keeps every value inside its field and
+ * model0 + n_frames <= 10^8.  coords, tmpl, box, angles and out are 4-byte aligned; n_frames*S > out_capacity is
+ * MKB_ERR_CAPACITY. */
+int mkb_pdb_encode(mkb_handle_t h, void *stream, const float *coords, int64_t frame_stride, int64_t n_frames,
+                   int64_t natoms, const uint8_t *tmpl, const float *box, const float *angles, int64_t box_stride,
+                   int64_t model0, uint8_t *out, int64_t out_capacity);
+
 /* K10 (SURVEY 8f row 3): the kernel of the `within` / `exwithin` atom selections, replaces within_distance
  * (moleculekit/atomselect_utils/atomselect_utils.pyx:612-653; called from atomselect/atomselect.py:243-251).
  * coords [n_atoms,3] float32 device (one frame, row-major); sel1 [n1] uint32 device = query atoms (NULL = all atoms,

@@ -1,7 +1,7 @@
 """Host plumbing shared by the trajectory file modules that decode and encode frames on the device (``dcd``,
-``netcdf``, ``trr``, ``mdcrd``, ``xyz``): the frame selection, the chunk planner of a frame list, the slab gather and
-the whole-frame stager into staging buffers, the double-buffered read -> copy -> decode loop, the writers' coords
-intake, the frame-minor layout check, and the double-buffered encode -> copy -> write loop."""
+``netcdf``, ``trr``, ``mdcrd``, ``xyz``, ``pdb``): the frame selection, the chunk planner of a frame list, the slab
+gather and the whole-frame stager into staging buffers, the double-buffered read -> copy -> decode loop, the writers'
+coords intake, the frame-minor layout check, and the double-buffered encode -> copy -> write loop."""
 from __future__ import annotations
 
 import os

@@ -48,10 +48,10 @@ enum ScratchSlot {
     S_TMSCORE_MASK, // K19: two cut-set bitmasks per resident thread
     S_MOMENT_TAB,   // K20: segment table, group offsets / totals and weights, uploaded per call
     S_MOMENT_PART,  // K20: per-(segment, frame) partial moment sums
-    S_XYZ_COUNTS,   // K26: newlines per 32 KB segment
-    S_XYZ_BASE,     // K26: number of the first newline of every segment
-    S_XYZ_STARTS,   // K26: line starts of the staged frames
-    S_XYZ_STATE,    // K26: the decode's running line count
+    S_XYZ_COUNTS,   // K26: newlines (K28: atom records) per 32 KB segment
+    S_XYZ_BASE,     // K26: number of the first newline (K28: atom record) of every segment
+    S_XYZ_STARTS,   // K26: line starts (K28: atom record starts) of the staged frames
+    S_XYZ_STATE,    // K26 / K28: the decode's running line (atom record) count
     S_BOND_MIN,     // K7: per-axis coordinate minimum (the reference's xyzmin) as order keys
     S_TMALIGN,      // K27: per-item traces, index lists and DP state of one item chunk
     S_NSLOTS

@@ -18,7 +18,7 @@
 //           stores only at the two ragged ends.  A tile owns the bytes of its values, the newline after each of them that
 //           ends a line and, for the last value tile, the box line: no two CTAs write the same byte.
 //
-// Arithmetic (the contract with Python's float() and '%8.3f'):
+// Arithmetic (the contract with Python's float() and '%8.3f'; md_parse / md_format in f83.cuh):
 //   decode  the digits k of the field (point removed, k < 10^7) give __double2float_rn((double)k / 1000.0), the sign
 //           applied afterwards: the double division is correctly rounded like float(), so both round the decimal once
 //           to double and once to float32, and '-0.000' gives -0.0.
@@ -27,6 +27,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "f83.cuh"
 #include "frame_tile.cuh"
 
 namespace mkb {
@@ -37,68 +38,6 @@ constexpr int MD_ROW = 812;                      // image row: the span plus 3 b
 static_assert(MD_ROW % 4 == 0 && MD_ROW >= MD_MAX_SPAN + 3 && (MD_ROW / 4) % 2 == 1, "image row");
 
 __device__ __forceinline__ long long md_pos(long long j) { return 8 * j + j / 10; }  // byte of value j in its frame
-
-// per byte: bit 7 set where the byte is not zero
-__device__ __forceinline__ unsigned md_nonzero(unsigned x) { return (((x & 0x7f7f7f7fu) + 0x7f7f7f7fu) | x) & 0x80808080u; }
-// per byte of x ^ '0000': bit 7 set where the byte is not a digit
-__device__ __forceinline__ unsigned md_nondigit(unsigned d) { return (((d & 0x7f7f7f7fu) + 0x76767676u) | d) & 0x80808080u; }
-
-// The 8 characters of a field as two little-endian words (lo: characters 0-3, hi: 4-7) -> float32 bits.  ok = the
-// field matches spaces, an optional '-', digits, '.', three digits.
-__device__ __forceinline__ unsigned md_parse(unsigned lo, unsigned hi, bool &ok) {
-    constexpr unsigned H = 0x80808080u;
-    const unsigned dl = lo ^ 0x30303030u, dh = hi ^ 0x30303030u;
-    const unsigned D = ~md_nondigit(dl) & H, Sp = ~md_nonzero(lo ^ 0x20202020u) & H, M = ~md_nonzero(lo ^ 0x2d2d2d2du) & H;
-    const unsigned smask = (Sp >> 7) * 0xffu;  // 0xff in every space byte
-    // the spaces are a prefix, a '-' (at most one) comes right after them, digits fill the rest
-    ok = (D | Sp | M) == H && (smask & (smask + 1u)) == 0u && (M == 0u || (M >> 7) == smask + 1u) &&
-         (hi & 0xffu) == 0x2eu && (md_nondigit(dh) & 0x80808000u) == 0u;
-    const unsigned v = dl & ((D >> 7) * 0xffu);  // digit values, 0 in the other bytes
-    const unsigned ip = (v & 0xffu) * 1000u + __dp4a(v, 0x010a6400u, 0u);
-    const unsigned k = ip * 1000u + __dp4a(dh, 0x010a6400u, 0u);
-    return __float_as_uint(__double2float_rn((double)k / 1000.0)) | (M ? 0x80000000u : 0u);
-}
-
-// The three aligned words covering bytes [a, a + 9) -> the field at a (lo, hi) and the byte at a + 8
-__device__ __forceinline__ void md_field(const unsigned char *a, unsigned &lo, unsigned &hi, unsigned &next) {
-    const unsigned *w = reinterpret_cast<const unsigned *>(reinterpret_cast<uintptr_t>(a) & ~uintptr_t(3));
-    const unsigned s = reinterpret_cast<uintptr_t>(a) & 3u;
-    const unsigned w0 = __ldg(w), w1 = __ldg(w + 1), w2 = __ldg(w + 2);
-    const unsigned sel = 0x3210u + 0x1111u * s;
-    lo = __byte_perm(w0, w1, sel);
-    hi = __byte_perm(w1, w2, sel);
-    next = (w2 >> (8 * s)) & 0xffu;
-}
-
-// float32 -> the 8 characters of '%8.3f' (lo: characters 0-3, hi: 4-7); '********' (Fortran's overflow field) outside
-// the writable range and for NaN / +-inf
-__device__ __forceinline__ void md_format(float x, unsigned &lo, unsigned &hi) {
-    const bool neg = signbit(x);
-    const double a = fabs(rint((double)x * 1000.0));
-    if (!(a <= (neg ? 999999.0 : 9999999.0))) {
-        lo = hi = 0x2a2a2a2au;
-        return;
-    }
-    const unsigned k = (unsigned)a, ip = k / 1000u, fp = k - 1000u * ip;
-    hi = 0x3030302eu + ((fp / 100u) << 8) + ((fp / 10u % 10u) << 16) + ((fp % 10u) << 24);
-    const unsigned digits = 0x30303030u + (ip / 1000u) + ((ip / 100u % 10u) << 8) + ((ip / 10u % 10u) << 16) +
-                            ((ip % 10u) << 24);
-    const int nd = ip >= 1000u ? 4 : ip >= 100u ? 3 : ip >= 10u ? 2 : 1;
-    const unsigned keep = 0xffffffffu << (8 * (4 - nd));  // the last nd characters
-    lo = (digits & keep) | (0x20202020u & ~keep);
-    if (neg) {  // nd <= 3 here: k <= 999 999
-        const int at = 8 * (3 - nd);
-        lo = (lo & ~(0xffu << at)) | (0x2du << at);
-    }
-}
-
-__device__ __forceinline__ void md_put(unsigned char *d, unsigned lo, unsigned hi) {
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-        d[c] = (unsigned char)(lo >> (8 * c));
-        d[4 + c] = (unsigned char)(hi >> (8 * c));
-    }
-}
 
 // coords[(a*3 + d)*frame_stride + k] = value a*3 + d of the frame at bytes + offsets[k]; with a box, box[d*box_stride + k]
 // = field d of its box line.  Every offset is a multiple of 4.

@@ -29,36 +29,15 @@
 
 #include "common.cuh"
 #include "frame_tile.cuh"
+#include "xl_lines.cuh"
 #include "xyz_number.cuh"
 
 namespace mkb {
 namespace {
 
-constexpr int XL_THREADS = 256, XL_ITEMS = 8;
-constexpr long long XL_SEG = 16LL * XL_THREADS * XL_ITEMS;  // bytes per segment (one CTA of the count and emit passes)
-constexpr int XL_SCAN_THREADS = 1024;
 constexpr int XYZ_COUNT_WINDOW = 64;  // bytes of a count line the device reads; a longer one is left to the host
 constexpr int XYZ_FIELD = 16;         // ' ' and a '%15.8f' field
 constexpr int XYZ_MAX_WIDTH = 256;    // widest element column the encoder takes
-
-// bit b of the result: byte b of the 16 bytes is c
-__device__ __forceinline__ unsigned xl_mask(const uint4 &v, unsigned c) {
-    const unsigned pat = c * 0x01010101u;
-    const unsigned w[4] = {v.x ^ pat, v.y ^ pat, v.z ^ pat, v.w ^ pat};
-    unsigned m = 0;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const unsigned z = ~((((w[i] & 0x7f7f7f7fu) + 0x7f7f7f7fu) | w[i])) & 0x80808080u;  // bit 7 of each zero byte
-        m |= (((z >> 7) & 1u) | ((z >> 14) & 2u) | ((z >> 21) & 4u) | ((z >> 28) & 8u)) << (4 * i);
-    }
-    return m;
-}
-
-// the bytes of the 16-byte word at p0 that lie below n
-__device__ __forceinline__ unsigned xl_valid(long long p0, long long n) {
-    const long long r = n - p0;
-    return r >= 16 ? 0xffffu : r <= 0 ? 0u : (1u << r) - 1u;
-}
 
 __global__ void __launch_bounds__(XL_THREADS) xyz_count_kernel(const uint4 *__restrict__ bytes, long long n,
                                                                unsigned *__restrict__ counts) {
@@ -73,24 +52,6 @@ __global__ void __launch_bounds__(XL_THREADS) xyz_count_kernel(const uint4 *__re
     }
     const unsigned total = Reduce(tmp).Sum(c);
     if (threadIdx.x == 0) counts[blockIdx.x] = total;
-}
-
-// base[s] = state[0] + the newlines of segments before s; state[0] += all of them
-__global__ void __launch_bounds__(XL_SCAN_THREADS) xyz_scan_kernel(const unsigned *__restrict__ counts, int n_seg,
-                                                                   long long *__restrict__ base,
-                                                                   long long *__restrict__ state) {
-    using Scan = cub::BlockScan<unsigned, XL_SCAN_THREADS>;  // a tile holds at most 1024 * 32 KB newlines
-    __shared__ typename Scan::TempStorage tmp;
-    long long carry = state[0];
-    for (int s0 = 0; s0 < n_seg; s0 += XL_SCAN_THREADS) {
-        const int s = s0 + threadIdx.x;
-        unsigned ex, total;
-        Scan(tmp).ExclusiveSum(s < n_seg ? counts[s] : 0u, ex, total);
-        if (s < n_seg) base[s] = carry + ex;
-        carry += total;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) state[0] = carry;
 }
 
 // the count line at b[p]: 0 when its first field is natoms written as [+]digits, else 1 (the host decides)
