@@ -492,6 +492,65 @@ int mkb_pdb_encode(mkb_handle_t h, void *stream, const float *coords, int64_t fr
                    int64_t natoms, const uint8_t *tmpl, const float *box, const float *angles, int64_t box_stride,
                    int64_t model0, uint8_t *out, int64_t out_capacity);
 
+/* K29: the index pass over a chunk of a multi-frame GROMACS GRO file; replaces the host reader's line loop as far as
+ * finding the frames.  The format: a frame is P = natoms + 3 lines -- a title (free text, GROMACS writes "t= <time>
+ * step= <step>" into it), the atom count (a free-format integer), natoms atom lines ("%5d%-5s%5s%5d": resid, resname,
+ * atom name, serial, then three position fields of width w in nm and optionally three velocity fields of width w in
+ * nm/ps) and a box line (free format: 3 values v1x v2y v3z or 9 values v1x v2y v3z v1y v1z v2x v2z v3x v3y, in nm).
+ * bytes = the chunk on the device, 16-byte aligned: the file's bytes [file_base, file_base + n_read), of which the
+ * newlines in the first n are counted (n_read - n bytes of look-ahead, up to 64, let the last count lines be checked).
+ * state (device int64[3], 8-byte aligned; the caller sets {0, INT64_MAX, 0} before the first chunk and keeps it across
+ * chunks, which run in file order on one stream): [0] the running newline count, [1] the atomic minimum file offset of
+ * a CR not followed by LF, [2] one more than the largest frame number past frame_cap.  Line L (0-based in the file)
+ * with L % P == 0 and L >= P that starts inside the look-ahead window gets frame_off[L / P] = its file offset; line L
+ * with L % P == 1 gets status[L / P] = 0 when its first field is natoms written as [+]digits (ASCII separators before
+ * it, a separator after it, within 64 bytes), 1 when the host must decide (frame_off, status device, frame_cap
+ * entries). */
+int mkb_gro_index(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t n, int64_t n_read, int64_t file_base,
+                  int64_t natoms, int64_t *state, int64_t *frame_off, uint8_t *status, int64_t frame_cap);
+
+/* K29: GRO frames parsed on the device; replaces the host reader's column slices and float() per atom line and the host
+ * transposition to the frame-minor arrays.  bytes = n_staged whole frames back to back on the device, 16-byte aligned,
+ * nbytes long and readable up to nbytes rounded up to 16; each frame's P = natoms + 3 lines end in '\n' (the last
+ * frame's last line may end at nbytes instead).  frame_of (HOST int32[n_frames]) = the staged frame of listed frame k.
+ * Atom line a must hold cols = 20 + 3 width characters (20 + 6 width when `velocities`, the file's velocity flag)
+ * before its '\n' or CRLF.  coords (natoms, 3, n_frames) float32 device, element (a, d, k) at coords[(a*3 + d)*
+ * frame_stride + k] = the width-character field at column 20 + width d of atom line a, bit for bit
+ * np.float32(float(field)); vels (NULL, or with `velocities` the same layout and stride) = the fields at column 20 +
+ * width (3 + d).  For width 8 the F8.3 (positions) and F8.4 (velocities) fast paths run first, else and for the fields
+ * they reject the grammar of mkb_xyz_decode within the field.  A short line, an empty field, a field outside the
+ * grammar, a byte >= 0x80 or an undecided rounding is flagged: flags (device int64, 8-byte aligned, flags[0] set to 0
+ * by the caller) receives (frame_base + k) * natoms + a at flags[1 + j] for j < flag_cap, and flags[0] counts every
+ * flagged line; such a line's values are unspecified.  1 <= width <= 32. */
+int mkb_gro_decode(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t nbytes, int64_t n_staged,
+                   const int32_t *frame_of, int64_t n_frames, int64_t natoms, int64_t width, int32_t velocities,
+                   float *coords, float *vels, int64_t frame_stride, int64_t frame_base, int64_t *flags,
+                   int64_t flag_cap);
+
+/* K29: the title and box lines of staged GRO frames parsed on the device.  Staged frame u is bytes[frame_at[u],
+ * frame_at[u + 1]) (bytes and frame_at device, frame_at int64[n_staged + 1]).  box (device float32[9 n_staged]): the
+ * ASCII-whitespace-separated tokens of the frame's last line in file order at box[9 u + t], each bit for bit
+ * np.float32(float(token)); time (device float64[n_staged]) = float() of the token after the first " t= " of the
+ * frame's first line, NaN without one; step (device int64[n_staged]) = the integer after the first " step= ", -1
+ * without one.  status (device int32[n_staged]): bit 0 when the box line does not hold 3 or 9 tokens or holds a token
+ * the device does not decide, bit 1 when the time token, bit 2 when the step token is left to the host ([+-] and at
+ * most 18 digits are decided); the values under a set bit are unspecified. */
+int mkb_gro_head(mkb_handle_t h, void *stream, const uint8_t *bytes, const int64_t *frame_at, int64_t n_staged,
+                 float *box, double *time, int64_t *step, int32_t *status);
+
+/* K29: GRO frames written on the device, the inverse of mkb_gro_decode.  coords float32 device, element (a, d, k) at
+ * coords[(a*3 + d)*frame_stride + k]; vels NULL or the same layout; box (3, 3, n_frames) float32 device, component j of
+ * box vector i at box[(3 i + j)*box_stride + k].  Frame k is written at out + k*S, S = head_bytes + natoms*L + B, L =
+ * 69 with vels else 45, B = 91 when box9 else 31: the head_bytes bytes head[k*head_bytes ...] (device: the frame's
+ * title and count lines), then per atom its 20 bytes prefix[a*20 ...] (device), '%8.3f' of x, y, z, with vels '%8.4f'
+ * of vx, vy, vz, and '\n'; then '%10.5f' of v1x v2y v3z (box9: and v1y v1z v2x v2z v3x v3y) and '\n'.  Each field is
+ * byte for byte Python's '%W.Df': rint(x * 10^D) in float64 (exact, half to even), the sign printed whenever x is
+ * negative or -0.0; the caller keeps every value inside its field.  coords, vels, prefix, box and out are 4-byte
+ * aligned; n_frames*S > out_capacity is MKB_ERR_CAPACITY. */
+int mkb_gro_encode(mkb_handle_t h, void *stream, const float *coords, const float *vels, int64_t frame_stride,
+                   int64_t n_frames, int64_t natoms, const uint8_t *head, int64_t head_bytes, const uint8_t *prefix,
+                   const float *box, int64_t box_stride, int32_t box9, uint8_t *out, int64_t out_capacity);
+
 /* K10 (SURVEY 8f row 3): the kernel of the `within` / `exwithin` atom selections, replaces within_distance
  * (moleculekit/atomselect_utils/atomselect_utils.pyx:612-653; called from atomselect/atomselect.py:243-251).
  * coords [n_atoms,3] float32 device (one frame, row-major); sel1 [n1] uint32 device = query atoms (NULL = all atoms,

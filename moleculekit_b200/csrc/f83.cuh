@@ -1,11 +1,12 @@
 // f83.cuh -- fixed-width decimal fields with SWAR code: Fortran F8.3 parsed and formatted (K25's mdcrd fields, K28's PDB
-// coordinate columns), and the general '%W.Df' formatter K28 uses for the CRYST1 fields.
+// coordinate columns, K29's GRO positions), F8.4 parsed (K29's GRO velocities), and the general '%W.Df' formatter K28
+// uses for the CRYST1 fields and K29 for the velocities and the box.
 //
 // Arithmetic (the contract with Python's float() and '%W.Df'):
 //   parse   the digits k of an F8.3 field (point removed, k < 10^7) give __double2float_rn((double)k / 1000.0), the sign
 //           applied afterwards: the double division is correctly rounded like float(), so both round the decimal once
 //           to double and once to float32, and '-0.000' gives -0.0.
-//   format  k = rint((double)x * 10^D) is exact before the rounding for D <= 3 (a float32 times 1000 fits 53 bits) and
+//   format  k = rint((double)x * 10^D) is exact before the rounding for D <= 12 (a float32 times 10^D fits 53 bits) and
 //           rounds half to even, which is what printf's correctly rounded '%.Df' does; the sign of x is printed even
 //           when k == 0.
 //
@@ -34,6 +35,22 @@ __device__ __forceinline__ unsigned md_parse(unsigned lo, unsigned hi, bool &ok)
     const unsigned ip = (v & 0xffu) * 1000u + __dp4a(v, 0x010a6400u, 0u);
     const unsigned k = ip * 1000u + __dp4a(dh, 0x010a6400u, 0u);
     return __float_as_uint(__double2float_rn((double)k / 1000.0)) | (M ? 0x80000000u : 0u);
+}
+
+// The 8 characters of an F8.4 field (GRO's '%8.4f' velocities; lo: characters 0-3, hi: 4-7) -> float32 bits.  ok =
+// the field matches spaces, an optional '-', digits (at most three characters before the point), '.' at character 3,
+// four digits; the value is __double2float_rn(k / 10000.0) of the seven digits k, as md_parse does for three decimals.
+__device__ __forceinline__ unsigned md_parse4(unsigned lo, unsigned hi, bool &ok) {
+    constexpr unsigned H = 0x00808080u;  // characters 0-2
+    const unsigned dl = lo ^ 0x30303030u, dh = hi ^ 0x30303030u;
+    const unsigned D = ~md_nondigit(dl) & H, Sp = ~md_nonzero(lo ^ 0x20202020u) & H, M = ~md_nonzero(lo ^ 0x2d2d2d2du) & H;
+    const unsigned smask = (Sp >> 7) * 0xffu;
+    ok = (D | Sp | M) == H && (smask & (smask + 1u)) == 0u && (M == 0u || (M >> 7) == smask + 1u) &&
+         (lo >> 24) == 0x2eu && md_nondigit(dh) == 0u;
+    const unsigned v = dl & ((D >> 7) * 0xffu);
+    const unsigned ip = __dp4a(v, 0x00010a64u, 0u);  // characters 0-2: 100, 10, 1
+    const unsigned k = ip * 10000u + (dh & 0xffu) * 1000u + __dp4a(dh, 0x010a6400u, 0u);
+    return __float_as_uint(__double2float_rn((double)k / 10000.0)) | (M ? 0x80000000u : 0u);
 }
 
 // The three aligned words covering bytes [a, a + 9) -> the field at a (lo, hi) and the byte at a + 8
@@ -77,13 +94,19 @@ __device__ __forceinline__ void md_put(unsigned char *d, unsigned lo, unsigned h
     }
 }
 
-// '%W.Df' of x into d[0 .. W), 1 <= D <= 3, the variant of md_format for other widths.  The caller has checked the
-// range: rint(x 10^D) < 10^(W - 1), 10^(W - 2) when x is negative, and x finite.
+__host__ __device__ constexpr double f_pow10(int d) { return d == 0 ? 1.0 : 10.0 * f_pow10(d - 1); }  // exact for d <= 22
+__host__ __device__ constexpr int f_bits(unsigned long long v) { return v ? 1 + f_bits(v >> 1) : 0; }
+__host__ __device__ constexpr unsigned long long f_pow5(int d) { return d == 0 ? 1ull : 5ull * f_pow5(d - 1); }
+
+// '%W.Df' of x into d[0 .. W), the variant of md_format for other widths.  The caller has checked the range: rint(x
+// 10^D) < 10^(W - 1), 10^(W - 2) when x is negative, and x finite.  x 10^D = x 2^D 5^D is exact in a double while the
+// float32's 24-bit significand times 5^D fits 53 bits (D <= 12), so rint rounds the exact product once.
 template <int W, int D>
 __device__ __forceinline__ void f_format(float x, unsigned char *d) {
-    static_assert(D >= 1 && D <= 3 && W >= D + 2 && W <= 16, "a float32 times 10^D must stay exact in a double");
+    static_assert(D >= 1 && 24 + f_bits(f_pow5(D)) <= 53 && W >= D + 2 && W <= 16,
+                  "a float32 times 10^D must stay exact in a double");
     const bool neg = signbit(x);
-    unsigned long long k = (unsigned long long)fabs(rint((double)x * (D == 1 ? 10.0 : D == 2 ? 100.0 : 1000.0)));
+    unsigned long long k = (unsigned long long)fabs(rint((double)x * f_pow10(D)));
 #pragma unroll
     for (int c = W - 1; c >= W - D; --c) {
         d[c] = (unsigned char)('0' + k % 10u);

@@ -17,6 +17,8 @@
 //               does them.  NaN is 0x7fc00000 with the token's sign, as np.float32(float('-nan')) gives.
 #pragma once
 
+#include <type_traits>
+
 #include "xyz_pow5.cuh"
 
 #ifdef __CUDACC__
@@ -59,6 +61,16 @@ XYZ_FN unsigned xyz_f32_bits(double d) {
     const float f = (float)d;  // to nearest even on the host's default rounding mode
     unsigned u;
     std::memcpy(&u, &f, 4);
+    return u;
+#endif
+}
+
+XYZ_FN unsigned long long xyz_f64_bits(double d) {
+#ifdef __CUDA_ARCH__
+    return (unsigned long long)__double_as_longlong(d);
+#else
+    unsigned long long u;
+    std::memcpy(&u, &d, 8);
     return u;
 #endif
 }
@@ -116,10 +128,10 @@ XYZ_FN unsigned long long xyz_lemire(long long q, unsigned long long w, bool *un
     return ((unsigned long long)p2 << 52) | m;
 }
 
-// The number starting at p -> *bits (float32); p is left on the byte after it.  false: not in the device grammar, or
-// undecided (the host re-reads the line).
-template <class R>
-XYZ_FN bool xyz_number(R &rd, long long &p, unsigned &bits) {
+// The number starting at p -> *bits (float32, or with F64 the float64 that float() gives); p is left on the byte after
+// it.  false: not in the device grammar, or undecided (the host re-reads the line).
+template <bool F64 = false, class R>
+XYZ_FN bool xyz_number(R &rd, long long &p, typename std::conditional<F64, unsigned long long, unsigned>::type &bits) {
     unsigned c = rd.at(p);
     bool neg = false;
     if (c == '+' || c == '-') {
@@ -137,11 +149,13 @@ XYZ_FN bool xyz_number(R &rd, long long &p, unsigned &bits) {
         }
         if (!xyz_sep(c)) return false;
         if (n == 3 && word == 0x6e616eull) {  // "nan"
-            bits = sign | 0x7fc00000u;
+            if constexpr (F64) bits = (unsigned long long)sign << 32 | 0x7ff8000000000000ull;
+            else bits = sign | 0x7fc00000u;
             return true;
         }
         if ((n == 3 && word == 0x696e66ull) || (n == 8 && word == 0x696e66696e697479ull)) {  // "inf", "infinity"
-            bits = sign | 0x7f800000u;
+            if constexpr (F64) bits = (unsigned long long)sign << 32 | 0x7ff0000000000000ull;
+            else bits = sign | 0x7f800000u;
             return true;
         }
         return false;
@@ -191,7 +205,8 @@ XYZ_FN bool xyz_number(R &rd, long long &p, unsigned &bits) {
     }
     if (!xyz_sep(c)) return false;
     if (w == 0) {
-        bits = sign;
+        if constexpr (F64) bits = (unsigned long long)sign << 32;
+        else bits = sign;
         return true;
     }
     double d;
@@ -210,7 +225,8 @@ XYZ_FN bool xyz_number(R &rd, long long &p, unsigned &bits) {
         }
         d = xyz_bits_f64(u);
     }
-    bits = sign | xyz_f32_bits(d);
+    if constexpr (F64) bits = (unsigned long long)sign << 32 | xyz_f64_bits(d);
+    else bits = sign | xyz_f32_bits(d);
     return true;
 }
 
