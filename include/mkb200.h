@@ -492,6 +492,56 @@ int mkb_pdb_encode(mkb_handle_t h, void *stream, const float *coords, int64_t fr
                    int64_t natoms, const uint8_t *tmpl, const float *box, const float *angles, int64_t box_stride,
                    int64_t model0, uint8_t *out, int64_t out_capacity);
 
+/* K30: the index pass over a chunk of the _atom_site loop body of a PDBx/mmCIF file; replaces the host reader's
+ * tokenizer as far as finding the frames.  The rules (the host applies them to what this pass returns):
+ *   - a line whose first non-blank byte is '#' (a comment) or '\n' is skipped; the body ends at the first line whose first
+ *     token is a tag ('_...'), loop_, stop_ or global_, or starts with data_ or save_ (letters in any case); every other
+ *     line is a row;
+ *   - blanks are space, \t, \v, \f and \r; a token is a run of other bytes, or a '...' / "..." string that opens at the
+ *     token's start and closes at the first matching quote followed by a blank or the line's end;
+ *   - a row holds exactly n_tags tokens, and its token model_col (when model_col >= 0) is an unquoted [+-]?digits of at
+ *     most 18 digits; a row starting with ';' (a text field) or with a quote that does not close is bad;
+ *   - a frame is a maximal run of rows with the same model number (model_col -1: the whole loop is one frame).
+ * bytes = the chunk on the device, 16-byte aligned: the file's bytes [file_base, file_base + n_read), of which the line
+ * starts after the newlines in the first n are classified (n_read - n bytes of look-ahead let the last rows be read
+ * whole); byte 0 starts a line when first != 0.  state (device int64[7], 8-byte aligned; the caller sets {0, INT64_MAX,
+ * 0, INT64_MAX, INT64_MAX, INT64_MIN, -1} before the first chunk and keeps it across chunks, which run in file order on
+ * one stream): [0] the running row count, [1] the minimum file offset of a CR not followed by LF before the body's end,
+ * [2] the number of marks, [3] the minimum file offset of a bad row, [4] the minimum file offset of a line that ends the
+ * body, [5] the model number of the last row so far (INT64_MIN: none), [6] the rows before the body's end once that
+ * line has been seen, else -1.  Every row before the body's end whose model number differs from the row before it
+ * appends (file offset, rows before it, model number) to marks (device int64[3 * mark_cap]) at slot state[2]++ while
+ * the slot is below mark_cap; the slots are in no particular order. */
+int mkb_cif_index(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t n, int64_t n_read, int64_t file_base,
+                  int64_t first, int64_t n_tags, int64_t model_col, int64_t *state, int64_t *marks, int64_t mark_cap);
+
+/* K30: mmCIF frames parsed on the device; replaces the host reader's tokenizer and float() of the Cartn_x, Cartn_y and
+ * Cartn_z tokens of every row and the host transposition to the frame-minor array.  bytes = n_staged whole frames back
+ * to back on the device, 16-byte aligned, nbytes long and readable up to nbytes rounded up to 16; each staged frame
+ * starts a line, holds exactly natoms rows (comment and blank lines between them are skipped, as by mkb_cif_index) and
+ * (but for the last) ends in '\n'.  frame_of (HOST int32[n_frames]) = the staged frame of listed frame k.  coords
+ * (natoms, 3, n_frames) float32 device, element (a, d, k) at coords[(a*3 + d)*frame_stride + k] = token col_x, col_y or
+ * col_z (0-based) of row a, bit for bit np.float32(float(token)) in the grammar of mkb_xyz_decode.  A quoted token, a
+ * token outside the grammar ('?', '.', '1.5(2)', ...), a byte >= 0x80 before the last of the three tokens, a row with
+ * fewer tokens or an undecided rounding is flagged as in mkb_pdb_decode: flags[1 + j] = (frame_base + k) * natoms + a for
+ * j < flag_cap, flags[0] counts every flagged row; such a row's coordinates are unspecified. */
+int mkb_cif_decode(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t nbytes, int64_t n_staged,
+                   const int32_t *frame_of, int64_t n_frames, int64_t natoms, int64_t col_x, int64_t col_y,
+                   int64_t col_z, float *coords, int64_t frame_stride, int64_t frame_base, int64_t *flags,
+                   int64_t flag_cap);
+
+/* K30: mmCIF rows written on the device, the inverse of mkb_cif_decode.  coords float32 device, element (a, d, k) at
+ * coords[(a*3 + d)*frame_stride + k].  Frame k is written at out + k*S, S = natoms*row_bytes: per atom the row_bytes of
+ * tmpl[a*row_bytes ...] (device, readable up to natoms*row_bytes rounded up to 4; row_bytes <= 768) with id =
+ * (frame0 + k)*natoms + a + 1 right-justified in id_width bytes at col_id, '%10.3f' of x, y and z at col_x, col_x + 11
+ * and col_x + 22, and pdbx_PDB_model_num = frame0 + k + 1 right-justified in model_width bytes at col_model.  Each field
+ * is byte for byte Python's '%10.3f' (as mkb_pdb_encode's fields); the caller keeps every value inside its field.  coords,
+ * tmpl and out are 4-byte aligned; n_frames*S > out_capacity is MKB_ERR_CAPACITY. */
+int mkb_cif_encode(mkb_handle_t h, void *stream, const float *coords, int64_t frame_stride, int64_t n_frames,
+                   int64_t natoms, const uint8_t *tmpl, int64_t row_bytes, int64_t col_id, int64_t id_width,
+                   int64_t col_x, int64_t col_model, int64_t model_width, int64_t frame0, uint8_t *out,
+                   int64_t out_capacity);
+
 /* K29: the index pass over a chunk of a multi-frame GROMACS GRO file; replaces the host reader's line loop as far as
  * finding the frames.  The format: a frame is P = natoms + 3 lines -- a title (free text, GROMACS writes "t= <time>
  * step= <step>" into it), the atom count (a free-format integer), natoms atom lines ("%5d%-5s%5s%5d": resid, resname,

@@ -1,5 +1,5 @@
 """Host plumbing shared by the trajectory file modules that decode and encode frames on the device (``dcd``,
-``netcdf``, ``trr``, ``mdcrd``, ``xyz``, ``pdb``): the frame selection, the chunk planner of a frame list, the slab
+``netcdf``, ``trr``, ``mdcrd``, ``xyz``, ``pdb``, ``gro``, ``cif``): the frame selection, the chunk planner of a frame list, the slab
 gather and the whole-frame stager into staging buffers, the double-buffered read -> copy -> decode loop, the writers'
 coords intake, the frame-minor layout check, and the double-buffered encode -> copy -> write loop."""
 from __future__ import annotations

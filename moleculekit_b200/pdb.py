@@ -40,7 +40,7 @@ The writer's per-frame layout is ``"MODEL %8d\\n"``, with a box ``"CRYST1%9.3f%9
 \\n"``, N atom lines of 80 columns and ``"ENDMDL\\n"``; the file ends with ``"END\\n"``.  A name of 4 characters starts in
 column 13, a shorter one in column 14 when the element has one letter, else in column 13; a resname of 4 characters
 fills columns 18-21, a shorter one is right-justified in 18-20.  Serials are written modulo 100 000, this writer's choice
-so that systems of any size can be written.  Not supported: CONECT / bonds, hybrid-36 serials, mmCIF, compressed files,
+so that systems of any size can be written.  Not supported: CONECT / bonds, hybrid-36 serials, compressed files,
 per-model topology differences and TER records in written files.
 """
 from __future__ import annotations
