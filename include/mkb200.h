@@ -542,6 +542,61 @@ int mkb_cif_encode(mkb_handle_t h, void *stream, const float *coords, int64_t fr
                    int64_t col_x, int64_t col_model, int64_t model_width, int64_t frame0, uint8_t *out,
                    int64_t out_capacity);
 
+/* K31: one BinaryCIF column decoded on the device; replaces a host reader's per-value loops over the column's encodings.
+ * data = the column's bytes on the device (16-byte aligned, nbytes long).  steps (HOST double[6 * n_steps]) = the
+ * encodings in decode order (the reverse of the file's list), six words each, unused words 0:
+ *   {1, type}                         ByteArray, first and only first: little-endian values, type Int8 1, Int16 2,
+ *                                     Int32 3, Uint8 4, Uint16 5, Uint32 6 (to 32-bit integers), Float32 32 or Float64 33
+ *                                     (to float32, rounded to nearest even); nbytes a multiple of the type's size;
+ *   {2, byteCount, isUnsigned, srcSize}   IntegerPacking (byteCount 1 or 2): an element equal to a limit (0xFF / 0xFFFF
+ *                                     unsigned, 0x7F or -0x80 / 0x7FFF or -0x8000 signed) is added to the next one;
+ *   {3, origin, srcType}              Delta: out[0] = origin + d[0], out[i] = out[i-1] + d[i] modulo 2^width(srcType);
+ *   {4, srcType, srcSize}             RunLength: (value, count) pairs, values narrowed to srcType;
+ *   {5, factor, srcType}              FixedPoint, last: float32(double(q) / factor);
+ *   {6, min, max, numSteps, srcType}  IntervalQuantization, last: float32(min + ((max - min) / (numSteps - 1)) * q), each
+ *                                     float64 operation rounded on its own.
+ * Integers wrap modulo 2^32; a Uint32 array keeps its values as unsigned.  Every array holds at most 2^31 - 2 values.
+ * mode 0 (rows): out[i] = decoded value i for i < n_out (int32 or float32 bits, 4-byte words).  mode 1 (frames): the
+ * column holds whole frames of natoms rows, floats; out[a*atom_stride + k] = value of row frames[k]*natoms + a for
+ * frames (HOST int64[n_out], any order, repeats allowed) and atom_stride >= n_out (an axis of (natoms, 3, F) frame-minor
+ * float32 coords: coords + axis*frame_stride with atom_stride = 3*frame_stride).  mode 2 (runs): integers; every row i
+ * whose value differs from row i-1 (and row 0) appends (i, value) to out (device int64[2 * n_out]) at slot status[1]++
+ * while the slot is below n_out, slots in no particular order.  status (device int64[2], 8-byte aligned, zeroed by the
+ * call): [0] 0, or the first data error found: 1 an IntegerPacking that ends inside a value, 2 one that holds another
+ * number of values than srcSize, 3 RunLength counts that do not sum to srcSize, 4 a negative count (the outputs are then
+ * unspecified); [1] the runs of mode 2.  A chain that does not fit these rules is MKB_ERR_BAD_ARG.  out is 4-byte
+ * aligned (mode 2: 8-byte).  Nothing is synchronised; the caller keeps data, out and status valid until the stream reaches the end. */
+int mkb_bcif_decode(mkb_handle_t h, void *stream, const uint8_t *data, int64_t nbytes, const double *steps,
+                    int64_t n_steps, int64_t mode, void *out, int64_t n_out, const int64_t *frames, int64_t natoms,
+                    int64_t atom_stride, int64_t *status);
+
+/* K31: q[k*natoms + a] = rint(double(x[a*atom_stride + k*frame_stride]) * factor) (half to even) for every atom a and
+ * frame k: one axis of a frame-minor (natoms, 3, F) float32 array (x = coords + axis*frame_stride, atom_stride =
+ * 3*frame_stride, frame stride 1) quantized in BinaryCIF's row order.  x and q (device int32[natoms * n_frames]) are
+ * 4-byte aligned; the caller keeps every value finite with its quantum inside int32. */
+int mkb_bcif_quantize(mkb_handle_t h, void *stream, const float *x, int64_t atom_stride, int64_t frame_stride,
+                      int64_t natoms, int64_t n_frames, double factor, int32_t *q);
+
+/* K31: the sizes of the BinaryCIF encoder's four chains of one int32 array, for the host to choose one.  The array has
+ * n values (1 to 2^31 - 2), value i = v[i % period] + (i / period) * step modulo 2^32 (v device int32[period], 4-byte
+ * aligned; step 0 and period n for a plain array).  Its deltas are d[0] = 0, d[i] = value i - value i-1 (modulo 2^32),
+ * and a run-length array is the (value, count) pairs of its maximal runs.  sizes (HOST int64[25]): [0] value 0, then
+ * for the chains (a) the array, (b) its run-length array, (c) its deltas, (d) their run-length array, six words each:
+ * length, minimum, and the elements IntegerPacking takes at 1 byte unsigned, 2 bytes unsigned, 1 byte signed and 2 bytes
+ * signed, each value v counting floor(|v| / |limit|) + 1 with the limit on v's side (unsigned sums count negative
+ * values as 0).  Synchronises the stream. */
+int mkb_bcif_sizes(mkb_handle_t h, void *stream, const int32_t *v, int64_t period, int64_t step, int64_t n,
+                   int64_t *sizes);
+
+/* K31: the payload of one chain of mkb_bcif_sizes's array (same v, period, step, n): chain 0 to 3 for (a) to (d) and
+ * n_packed its length as mkb_bcif_sizes reported it.  width 4 writes the chain's array as little-endian int32 (ByteArray
+ * Int32, 4 * n_packed bytes); width 1 or 2 writes it IntegerPacked (signed, or with is_unsigned unsigned: the caller
+ * checked that no value is negative) as little-endian Int8 / Int16 / Uint8 / Uint16 elements, as many as
+ * mkb_bcif_sizes counted.  out (device, 4-byte aligned) holds out_bytes; elements past it are not written, and width 4
+ * with 4 * n_packed > out_bytes is MKB_ERR_CAPACITY.  Nothing is synchronised. */
+int mkb_bcif_emit(mkb_handle_t h, void *stream, const int32_t *v, int64_t period, int64_t step, int64_t n, int64_t chain,
+                  int64_t width, int64_t is_unsigned, int64_t n_packed, uint8_t *out, int64_t out_bytes);
+
 /* K29: the index pass over a chunk of a multi-frame GROMACS GRO file; replaces the host reader's line loop as far as
  * finding the frames.  The format: a frame is P = natoms + 3 lines -- a title (free text, GROMACS writes "t= <time>
  * step= <step>" into it), the atom count (a free-format integer), natoms atom lines ("%5d%-5s%5s%5d": resid, resname,

@@ -51,7 +51,7 @@ The writer's file is ``data_<title>``, ``#``, with a box the six ``_cell`` items
 'P 1'``, ``#``, ``loop_`` and the 21 tags of :data:`TAGS` (RCSB's order), one row per atom and frame, and a last ``#``
 line.  Every column is padded to its widest value over the file (text left-justified, numbers right-justified) and
 separated by one space, so every frame has the same size; ``id`` = f N + a + 1 is unique across the file,
-``pdbx_PDB_model_num`` = f + 1.  Not supported: BinaryCIF, rows that span lines and ``;`` text fields in the loop, data
+``pdbx_PDB_model_num`` = f + 1.  Not supported: rows that span lines and ``;`` text fields in the loop, data
 blocks after the first, per-model topology differences, compressed files, and on write ``_atom_site_anisotrop``, bonds
 and ``_chem_comp``.
 """

@@ -54,6 +54,9 @@ enum ScratchSlot {
     S_XYZ_STATE,    // K26 / K28: the decode's running line (atom record) count
     S_BOND_MIN,     // K7: per-axis coordinate minimum (the reference's xyzmin) as order keys
     S_TMALIGN,      // K27: per-item traces, index lists and DP state of one item chunk
+    S_BCIF_VAL,     // K31: two 32-bit value arrays of a column's decode or encode, used in turn
+    S_BCIF_IDX,     // K31: int64 scans (value ranks, run starts, packed offsets)
+    S_BCIF_TMP,     // K31: cub temp storage and the listed frames
     S_NSLOTS
 };
 
