@@ -720,7 +720,10 @@ int mkb_hbonds_fill(mkb_handle_t h, void *stream, const mkb_traj *t, const uint3
  * int32 device = (ring index, second ring index | cation atom | halogen atom) and distangles [total][2] float32 device =
  * (distance, angle in degrees), in the reference's order (frame, ring, partner ascending).  Pairs and distances are the
  * reference binary's; the reported angle is within a few ulp (it comes from the device's acos, the reference's from glibc's
- * acosf). */
+ * acosf).  Every ring must have at least 3 atoms: its normal comes from its first three.  The reference reads atoms of the
+ * next ring (or past the end of rings_atoms) for a shorter ring, so it has no defined answer; the Python wrappers reject
+ * one with a ValueError, and these entry points, which do not read the start indexes on the host, give it a zero normal
+ * (dot products 0). */
 int mkb_ring_pairs_count(mkb_handle_t h, void *stream, int32_t mode, const mkb_traj *t, const uint32_t *rings_atoms,
                          const uint32_t *starts1, int64_t n_rings1, const uint32_t *second, int64_t n_second, float p0,
                          float p1, float p2, float p3, int64_t *row_offsets, int64_t *total_pairs);

@@ -143,7 +143,8 @@ __global__ void hb_set_last_zero(long long *p, long long n) {
 }
 
 // largest float c in [-1, 1] with acosf(c) > athr (host libm = the reference's); -inf when none.  glibc's acosf is
-// non-increasing over all 2.13e9 floats of [-1, 1] (checked exhaustively on glibc 2.39), so one bound is exact.
+// non-increasing over all 2.13e9 floats of [-1, 1] (tests/test_interaction_cutoffs_cpu.py walks them all with the host
+// libm), so one bound is exact.
 static float hb_cos_threshold(float athr) {
     auto passes = [&](float c) { return acosf(c) > athr; };
     if (!passes(-1.f)) return -INFINITY;

@@ -83,7 +83,9 @@ __global__ void ring_prep_kernel(const float *__restrict__ coords, long long fs,
 #pragma unroll
     for (int i = 0; i < 3; ++i) m[i] = __fdiv_rn(m[i], cnt);
     float a[3] = {0.f, 0.f, 0.f}, nrm[3] = {0.f, 0.f, 0.f};
-    if (e - s >= 3) {  // the reference reads atoms s, s + 1, s + 2 whatever the ring size; rings have >= 3 atoms
+    // The reference reads atoms s, s + 1, s + 2 whatever the ring size.  The Python wrappers reject rings of fewer than 3
+    // atoms; a caller of the C entry points that passes one gets a zero normal here rather than another ring's atoms.
+    if (e - s >= 3) {
         const float *p0 = coords + (long long)atoms[s] * 3 * fs + f, *p1 = coords + (long long)atoms[s + 1] * 3 * fs + f,
                     *p2 = coords + (long long)atoms[s + 2] * 3 * fs + f;
         float t1[3], t2[3];

@@ -186,6 +186,13 @@ def waterbridge_calculate(mol, donors, acceptors, sel1, sel2, order: int = 1, di
     return water_bridges
 
 
+def _check_rings(name, rings):
+    """rings of fewer than 3 atoms have no normal (the reference reads the next ring's atoms for one): rejected"""
+    for i, rr in enumerate(rings):
+        if len(rr) < 3:
+            raise ValueError(f"{name}[{i}] has {len(rr)} atoms; rings need at least 3")
+
+
 def _ring_lists(mol, rings, off, pairs, da, return_rings, second_rings=None):
     index_list, dist_ang_list = [], []
     for f in range(mol.numFrames):
@@ -206,6 +213,8 @@ def pipi_calculate(mol, rings1, rings2, dist_threshold1: float = 4.4, angle_thre
 
     if angle_threshold1_max < 0 or angle_threshold1_max > 90 or angle_threshold2_min < 0 or angle_threshold2_min > 90:
         raise RuntimeError("Values for angles should be [0, 90] degrees")
+    _check_rings("rings1", rings1)
+    _check_rings("rings2", rings2)
     if len(rings1) == 0 or len(rings2) == 0:
         return [[] for _ in range(mol.numFrames)], [[] for _ in range(mol.numFrames)]
     ring_atoms = np.hstack((np.hstack(rings1), np.hstack(rings2)))
@@ -226,6 +235,7 @@ def cationpi_calculate(mol, rings, cations, dist_threshold: float = 5, angle_thr
 
     if angle_threshold_min < 0 or angle_threshold_min > 90:
         raise RuntimeError("Values for angles should be [0, 90] degrees")
+    _check_rings("rings", rings)
     if len(rings) == 0 or len(cations) == 0:
         return [[] for _ in range(mol.numFrames)], [[] for _ in range(mol.numFrames)]
     ring_atoms = np.hstack(rings)
@@ -245,6 +255,7 @@ def sigmahole_calculate(mol, rings, halides, dist_threshold: float = 4.5, angle_
 
     if angle_threshold_min < 0 or angle_threshold_min > 90:
         raise RuntimeError("Values for angles should be [0, 90] degrees")
+    _check_rings("rings", rings)
     if len(rings) == 0 or len(halides) == 0:
         return [[] for _ in range(mol.numFrames)], [[] for _ in range(mol.numFrames)]
     ring_atoms = np.hstack(rings)

@@ -44,13 +44,27 @@ def calculate_device(mode: int, coords, box, rings_atoms, starts1, second, p0, p
     return frame_off.contiguous(), pairs, da
 
 
+def check_ring_sizes(name, starts):
+    """Every ring needs at least 3 atoms: its normal comes from the first three.  The reference reads atoms of the next ring
+    (or past the end of the atom list) for a shorter one, so such a ring has no defined answer and is rejected."""
+    sizes = np.diff(np.asarray(starts, dtype=np.int64))
+    bad = np.flatnonzero(sizes < 3)
+    if bad.size:
+        i = int(bad[0])
+        raise ValueError(f"ring {i} of {name} has {int(sizes[i])} atoms; rings need at least 3")
+
+
 def calculate_arrays(mode, rings_atoms, starts1, second, coords, box, p0, p1=0.0, p2=0.0, p3=0.0, device=None):
-    """(frame_offsets (F+1,), pairs (total, 2) int32 -- partner atoms as ORIGINAL indexes --, distangles (total, 2) float32)."""
+    """(frame_offsets (F+1,), pairs (total, 2) int32 -- partner atoms as ORIGINAL indexes --, distangles (total, 2) float32).
+    Raises ValueError for a ring of fewer than 3 atoms."""
     _check("rings_atoms", rings_atoms, np.uint32, 1); _check("rings_start_indexes", starts1, np.uint32, 1)
     _check("coords", coords, np.float32, 3); _check("box", box, np.float32, 2)
     second = np.ascontiguousarray(second)
     if second.dtype != np.uint32:
         raise ValueError("Buffer dtype mismatch, expected 'uint32'")
+    check_ring_sizes("rings_start_indexes" if mode != PIPI else "rings1_start_indexes", starts1)
+    if mode == PIPI:
+        check_ring_sizes("rings2_start_indexes", second)
     F = coords.shape[2]
     n1 = len(starts1) - 1
     n2 = len(second) - 1 if mode == PIPI else len(second)

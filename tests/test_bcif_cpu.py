@@ -2,7 +2,6 @@
 independent oracle's encoders against its decoders on the packing limits and int32 wrap, the size formula against the
 packed lengths, the classifier's tie order, the container errors raised before any device call, every writer check
 before the file is opened, and the C-ABI symbols."""
-import gzip
 import os
 
 import msgpack
@@ -79,7 +78,8 @@ def _doc(cats, blocks=None):
 @pytest.mark.parametrize("raw,match", [
     (b"", "not a \\(gzip\\) MessagePack"),
     (b"\xc1garbage", "not a \\(gzip\\) MessagePack"),
-    (gzip.compress(b"\xc1"), "not a \\(gzip\\) MessagePack"),
+    # gzip of b"\xc1" written out with a zero timestamp, so the test id is the same on every run and every Python
+    (b"\x1f\x8b\x08\x00\x00\x00\x00\x00\x02\xff;\x08\x00\xab\x1da>\x01\x00\x00\x00", "not a \\(gzip\\) MessagePack"),
     (msgpack.packb([1, 2, 3]), "not shaped as a BinaryCIF document"),
     (_doc(None, blocks=[]), "not shaped"),
     (_doc([{"name": "_atom_site", "columns": [{"name": 3, "data": {}}], "rowCount": 1}]), "not shaped"),
