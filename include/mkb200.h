@@ -656,6 +656,72 @@ int mkb_gro_encode(mkb_handle_t h, void *stream, const float *coords, const floa
                    int64_t n_frames, int64_t natoms, const uint8_t *head, int64_t head_bytes, const uint8_t *prefix,
                    const float *box, int64_t box_stride, int32_t box9, uint8_t *out, int64_t out_capacity);
 
+/* K32: the index pass over a chunk of a LAMMPS dump file (dump atom / dump custom text); replaces the host reader's
+ * line loop as far as finding and checking the frames.  A frame is P = H + natoms lines: H header lines (ITEM: TIME and
+ * its value, ITEM: TIMESTEP and its value, ITEM: NUMBER OF ATOMS and the count, ITEM: BOX BOUNDS and three bound lines,
+ * ITEM: ATOMS and its column names, in frame 0's order) and natoms atom lines; frame 0 may start with an ITEM: UNITS
+ * pair the later frames lack.  bytes = the chunk on the device, 16-byte aligned: the file's bytes [file_base, file_base
+ * + n_read), of which the newlines in the first n are counted (the look-ahead lets a header that starts in the chunk
+ * be checked).  tmpl (device) = frame 0's H header lines without trailing blanks or CR, each ended by '\n';
+ * count_line (0 <= count_line < H) = the header line holding the atom count.  state (device int64[4], 8-byte aligned;
+ * the caller sets {-u, INT64_MAX, 0, 0} before the first chunk, u = the lines of frame 0's UNITS pair, and keeps it
+ * across chunks, which run in file order on one stream): [0] the running newline count minus u, [1] the atomic minimum
+ * file offset of a CR not followed by LF, [2] one more than the largest frame number past frame_cap, [3] scratch.
+ * Frame f >= 1 starts at line L = f P (lines counted from the first after the UNITS pair): frame_off[f] = its file
+ * offset, status[f] = 0 when each ITEM line of its header equals tmpl's byte for byte (trailing blanks and CR allowed)
+ * and its count line is natoms ([+-]digits between blanks), 1 when the host must decide -- a mismatch or a header that
+ * runs past n_read (frame_off, status device, frame_cap entries).  frame_off[0] is set only with u > 0. */
+int mkb_lammpstrj_index(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t n, int64_t n_read,
+                        int64_t file_base, int64_t P, int64_t natoms, const uint8_t *tmpl, int64_t H,
+                        int64_t count_line, int64_t *state, int64_t *frame_off, uint8_t *status, int64_t frame_cap);
+
+/* K32: the header values of the LAMMPS dump frames that start in a chunk, parsed on the device after
+ * mkb_lammpstrj_index on the same chunk, state and frame_off (same bytes, n, n_read, file_base and P).  Lines are
+ * counted from the frame's first: step_line holds TIMESTEP ([+-] and at most 18 digits), time_line (-1: none) TIME,
+ * box_line .. box_line + 2 the bound lines of 2 + ntilt values each (ntilt 0 or 1).  Frame f >= 1 of the chunk gets
+ * step[f] (int64), time[f] (float64) and bounds[9 f + 3 i + j] (float64: line i's lo, hi and, with ntilt, tilt; 0
+ * without), every value float() of its token (the grammar of mkb_xyz_decode); hstatus[f] = 1 when a line is left to
+ * the host (another token or token count, or a line past n_read), its values then unspecified.  All device arrays of
+ * frame_cap entries. */
+int mkb_lammpstrj_head(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t n, int64_t n_read,
+                       int64_t file_base, int64_t P, const int64_t *state, const int64_t *frame_off, int64_t frame_cap,
+                       int64_t step_line, int64_t time_line, int64_t box_line, int64_t ntilt, int64_t *step,
+                       double *time, double *bounds, uint8_t *hstatus);
+
+/* K32: LAMMPS dump atom lines parsed on the device and placed by id; replaces the host reader's split(), float() and
+ * int() per atom line, the sort by id and the transposition to the frame-minor arrays.  bytes = n_staged whole frames
+ * of P = H + natoms lines back to back on the device (16-byte aligned, readable up to nbytes rounded up to 16), each
+ * line ending in '\n' except possibly the last.  frame_of (HOST int32[n_frames]) = the staged frame of listed frame k.
+ * role (device int8[n_cols]) = what column c of an atom line is: 0 skipped (its bytes < 0x80), 1 the id, 2-4 the
+ * coordinate triple, 5-7 the image flags, 8-10 vx vy vz, 11-13 fx fy fz; columns past n_cols are not read.  ids NULL:
+ * row = id - 1 (ids 1..natoms; without an id column row = the line's rank); else ids (device int64[natoms], ascending)
+ * is searched for the row.  params (device float64[9 n_frames]): xlo ylo zlo lx ly lz xy xz yz of listed frame k.  Every
+ * value is float() of its token in float64 (the grammar of mkb_xyz_decode; ids and image flags [+-] and at most 18
+ * digits); with `scaled` x = ((xlo + xs lx) + ys xy) + zs xz, y = (ylo + ys ly) + zs yz, z = zlo + zs lz, with
+ * `unwrap` x += (ix lx + iy xy) + iz xz, y += iy ly + iz yz, z += iz lz, each step a correctly rounded float64
+ * operation, then one rounding to float32: coords (NULL: none) element (row, d, k) at coords[(row*3 + d)*frame_stride
+ * + k]; vels and forces (NULL: none) the same layout.  fstat (device uint8, 4-byte aligned, n_frames rounded up to 4
+ * entries; set to 0 here): bit 0 of fstat[k] when a line of listed frame k is left to the host (a short line, a token
+ * outside the grammar, a byte >= 0x80, an undecided rounding), bit 1 when an id is unknown or seen twice; that frame's
+ * rows are then unspecified. */
+int mkb_lammpstrj_decode(mkb_handle_t h, void *stream, const uint8_t *bytes, int64_t nbytes, int64_t n_staged,
+                         const int32_t *frame_of, int64_t n_frames, int64_t natoms, int64_t H, const int8_t *role,
+                         int64_t n_cols, const int64_t *ids, const double *params, int32_t scaled, int32_t unwrap,
+                         float *coords, float *vels, float *forces, int64_t frame_stride, uint8_t *fstat);
+
+/* K32: LAMMPS dump frames written on the device, the inverse of mkb_lammpstrj_decode for '%d %d %.9g %.9g %.9g'
+ * lines.  coords float32 device, element (a, d, k) at coords[(a*3 + d)*frame_stride + k]; vels NULL or the same
+ * layout.  ids, types (device int64[natoms]).  head (device) holds the n_frames frame headers back to back, frame k's at
+ * [head_off[k], head_off[k + 1]) (head_off device int64[n_frames + 1], head_off[0] = 0, head_bytes = head_off[n_frames]).
+ * Frame k is its header and then per atom '%d %d' of ids[a] and types[a], ' %.9g' of x, y, z (and with vels of vx, vy,
+ * vz) and '\n', byte for byte Python's '%.9g' % float(v) (nan, inf, -inf as Python spells them), the frames back to
+ * back from out.  A length pass, a scan and an emit pass: *total (device int64) receives the bytes written.  line_max
+ * is the caller's bound on one atom line; head_bytes + n_frames*natoms*line_max > out_capacity is MKB_ERR_CAPACITY. */
+int mkb_lammpstrj_encode(mkb_handle_t h, void *stream, const float *coords, const float *vels, int64_t frame_stride,
+                         int64_t n_frames, int64_t natoms, const int64_t *ids, const int64_t *types, int64_t line_max,
+                         const uint8_t *head, const int64_t *head_off, int64_t head_bytes, uint8_t *out,
+                         int64_t out_capacity, int64_t *total);
+
 /* K10 (SURVEY 8f row 3): the kernel of the `within` / `exwithin` atom selections, replaces within_distance
  * (moleculekit/atomselect_utils/atomselect_utils.pyx:612-653; called from atomselect/atomselect.py:243-251).
  * coords [n_atoms,3] float32 device (one frame, row-major); sel1 [n1] uint32 device = query atoms (NULL = all atoms,

@@ -47,6 +47,7 @@ EXPORTS = [
     "mkb_xyz_decode", "mkb_xyz_encode", "mkb_pdb_index", "mkb_pdb_decode", "mkb_pdb_cell", "mkb_pdb_encode",
     "mkb_gro_index", "mkb_gro_decode", "mkb_gro_head", "mkb_gro_encode", "mkb_cif_index", "mkb_cif_decode",
     "mkb_cif_encode", "mkb_bcif_decode", "mkb_bcif_quantize", "mkb_bcif_sizes", "mkb_bcif_emit",
+    "mkb_lammpstrj_index", "mkb_lammpstrj_head", "mkb_lammpstrj_decode", "mkb_lammpstrj_encode",
     "mkb_wrap_triclinic", "mkb_hbonds_count", "mkb_hbonds_fill", "mkb_ring_pairs_count", "mkb_ring_pairs_fill",
     "mkb_align_fit", "mkb_align_apply", "mkb_rmsd", "mkb_coordinates", "mkb_coord_sums", "mkb_fluctuation",
     "mkb_frame_moments", "mkb_dihedrals", "mkb_sasa", "mkb_sasa_chunk_frames", "mkb_dssp", "mkb_dssp_chunk_frames",
@@ -147,6 +148,11 @@ def load():
     lib.mkb_bcif_quantize.argtypes = [vp, vp, vp, i64, i64, i64, i64, dbl, vp]
     lib.mkb_bcif_sizes.argtypes = [vp, vp, vp, i64, i64, i64, vp]
     lib.mkb_bcif_emit.argtypes = [vp, vp, vp, i64, i64, i64, i64, i64, i64, i64, vp, i64]
+    lib.mkb_lammpstrj_index.argtypes = [vp, vp, vp, i64, i64, i64, i64, i64, vp, i64, i64, vp, vp, vp, i64]
+    lib.mkb_lammpstrj_head.argtypes = [vp, vp, vp, i64, i64, i64, i64, vp, vp, i64, i64, i64, i64, i64, vp, vp, vp, vp]
+    lib.mkb_lammpstrj_decode.argtypes = [vp, vp, vp, i64, i64, vp, i64, i64, i64, vp, i64, vp, vp, i32, i32, vp, vp,
+                                         vp, i64, vp]
+    lib.mkb_lammpstrj_encode.argtypes = [vp, vp, vp, vp, i64, i64, i64, vp, vp, i64, vp, vp, i64, vp, i64, vp]
     lib.mkb_wrap_box.argtypes = [vp, vp, tp, vp, i64, vp, i64, C.POINTER(C.c_float)]
     lib.mkb_wrap_triclinic.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, i64, C.POINTER(C.c_float), i32]
     lib.mkb_hbonds_count.argtypes = [vp, vp, tp, vp, i64, vp, i64, vp, vp, f32, f32, i32, i32, vp, C.POINTER(i64)]

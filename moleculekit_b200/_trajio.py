@@ -1,5 +1,5 @@
 """Host plumbing shared by the trajectory file modules that decode and encode frames on the device (``dcd``,
-``netcdf``, ``trr``, ``mdcrd``, ``xyz``, ``pdb``, ``gro``, ``cif``): the frame selection, the chunk planner of a frame list, the slab
+``netcdf``, ``trr``, ``mdcrd``, ``xyz``, ``pdb``, ``gro``, ``cif``, ``lammpstrj``): the frame selection, the chunk planner of a frame list, the slab
 gather and the whole-frame stager into staging buffers, the double-buffered read -> copy -> decode loop, the writers'
 coords intake, the frame-minor layout check, and the double-buffered encode -> copy -> write loop."""
 from __future__ import annotations
@@ -141,10 +141,11 @@ def frame_minor(coords: torch.Tensor) -> torch.Tensor:
 
 
 def write_encoded(fh, dev, n_frames: int, frame_bytes: int, chunk_bytes: int, encode) -> None:
-    """Write ``n_frames`` records of ``frame_bytes`` each to ``fh``, encoded on ``dev`` in chunks of at most
-    ``chunk_bytes`` (one frame at least): ``encode(f0, f1, out)`` enqueues frames [f0, f1) into the uint8 device buffer
-    ``out`` on the current stream.  Two device and two pinned buffers: each chunk is copied to the host and written
-    while the next one encodes."""
+    """Write ``n_frames`` records of ``frame_bytes`` each (at most, for records of variable size) to ``fh``, encoded on
+    ``dev`` in chunks of at most ``chunk_bytes`` (one frame at least): ``encode(f0, f1, out)`` enqueues frames [f0, f1)
+    into the uint8 device buffer ``out`` on the current stream; an int it returns is the bytes it wrote, anything else
+    means the records fill (f1 - f0) * frame_bytes bytes.  Two device and two pinned buffers: each chunk is copied to the host and
+    written while the next one encodes."""
     S = frame_bytes
     per = max(1, min(n_frames, int(chunk_bytes) // S))
     spans = [(f0, min(n_frames, f0 + per)) for f0 in range(0, n_frames, per)]
@@ -156,8 +157,8 @@ def write_encoded(fh, dev, n_frames: int, frame_bytes: int, chunk_bytes: int, en
     pending = None  # (buffer, bytes) copied to the host but not yet written
     for c, (f0, f1) in enumerate(spans):
         i = c % n_buf
-        encode(f0, f1, devb[i])
-        nbytes = (f1 - f0) * S
+        used = encode(f0, f1, devb[i])
+        nbytes = used if isinstance(used, int) else (f1 - f0) * S
         host[i][:nbytes].copy_(devb[i][:nbytes], non_blocking=True)
         done[i] = torch.cuda.Event()
         done[i].record(stream)

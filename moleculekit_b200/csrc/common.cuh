@@ -57,6 +57,9 @@ enum ScratchSlot {
     S_BCIF_VAL,     // K31: two 32-bit value arrays of a column's decode or encode, used in turn
     S_BCIF_IDX,     // K31: int64 scans (value ranks, run starts, packed offsets)
     S_BCIF_TMP,     // K31: cub temp storage and the listed frames
+    S_LMP_BITMAP,   // K32: one bit per (listed frame, atom row) of a decode: the ids seen
+    S_LMP_LEN,      // K32: line lengths and their exclusive scan of an encode
+    S_LMP_TMP,      // K32: cub temp storage of the encode's scan
     S_NSLOTS
 };
 
