@@ -50,7 +50,7 @@ import torch
 
 from . import _lib, _trajio
 from .cif import CELL, TAGS
-from .pdb import FIELDS, _fields, _first_bad, _name
+from .pdb import FIELDS, topology_fields
 
 TYPE_BYTES = {1: 1, 2: 2, 3: 4, 4: 1, 5: 2, 6: 4, 32: 4, 33: 8}
 INT_TYPES = (1, 2, 3, 4, 5, 6)
@@ -283,7 +283,7 @@ def index_bcif(filename, device=None) -> dict:
     each frame's pdbx_PDB_model_num, 0 without the column), topology (frame 0's rows, ``pdb.FIELDS`` keys), box and
     boxangles ((3,) float32: the file's one cell), columns (the ``_atom_site`` columns by lower-case name, as read),
     rows (its rowCount)).  Errors: see the module docstring."""
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     cats = _load(fn)
     if "atom_site" not in cats:
         raise ValueError(f"BinaryCIF file {fn}: no _atom_site category in the first data block")
@@ -335,7 +335,7 @@ def decode_bcif_device(data: dict, rows: int | None = None, device=None) -> torc
 
 
 def _read(filename, frames, index, device):
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     idx = index if index is not None else index_bcif(fn, device)
     N, F, rows = int(idx["natoms"]), int(idx["n_frames"]), int(idx["rows"])
     sel = _trajio.select(F, frames)
@@ -431,7 +431,7 @@ def encode_bcif_device(values: torch.Tensor, factor: int | None = None) -> tuple
         data, enc = _encode_ints(values.contiguous(), values.numel())
     else:
         x = values.to(torch.float32)
-        bad = _first_bad(x.reshape(1, 1, -1), *INT32, factor)
+        bad = _trajio.first_bad(x.reshape(1, 1, -1), *INT32, factor)
         if bad is not None:
             raise ValueError(f"values[{bad[0]}] = {bad[3]!r}: rint(x * {factor}) must be a finite int32")
         q = torch.empty(x.numel(), dtype=torch.int32, device=dev)
@@ -502,7 +502,7 @@ def _prepare(coords, topology, box, boxangles, title, device):
     box, angles = cell
     if box is not None and angles is None:
         angles = np.full((3, F), 90.0, np.float32)
-    t = _fields(topology, natoms)
+    t = topology_fields(topology, natoms)
     bad = []
     for k in ("record", "name", "altloc", "resname", "chain", "insertion", "segid", "element"):
         vals = t[k].tolist()
@@ -524,7 +524,7 @@ def _prepare(coords, topology, box, boxangles, title, device):
     if bad:
         a, k, why = min(bad)
         raise ValueError(f"topology at atom {a}, field {k} is {why}")
-    b = _first_bad(coords, *INT32, 1000)
+    b = _trajio.first_bad(coords, *INT32, 1000)
     if b is not None:
         f, atom, axis, v = b
         raise ValueError(f"coords at frame {f}, atom {atom}, axis {'xyz'[axis]} is {v!r}: FixedPoint(1000) holds "
@@ -600,7 +600,7 @@ def write_bcif(filename, coords, topology, box=None, boxangles=None, title=None,
     with rint(x * 1000) inside int32; box and angles likewise (1000, 100) and equal in every frame; text ASCII strings;
     resid and charge int32 integers; occupancy and beta finite with rint(x * 100) inside int32.  The layout is in the
     module docstring.  The file is created or truncated."""
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     raw = bcif_bytes(coords, topology, box, boxangles, title, device)
     with open(fn, "wb") as fh:
         fh.write(raw)

@@ -67,8 +67,9 @@ import numpy as np
 import torch
 
 from . import _lib, _trajio
-from .pdb import FIELDS, _fields, _first_bad, _name
-from .xyz import _line_at, _line_col
+from .pdb import FIELDS, topology_fields
+
+_fields = topology_fields  # the name bench_cif.py and the tests build writer layouts with
 
 logger = logging.getLogger(__name__)
 
@@ -207,11 +208,11 @@ def _scan(fn, fd: int, pos: int, E: int, find_loop: bool) -> dict:
                 try:
                     cell[name] = _value(*parts[1])
                 except ValueError:
-                    raise ValueError(f"CIF file {fn}, line {_line_col(fd, at)[0] + 1}: _cell.{name} "
+                    raise ValueError(f"CIF file {fn}, line {_trajio.line_col(fd, at)[0] + 1}: _cell.{name} "
                                      f"{parts[1][0]!r} is not a number") from None
         elif find_loop and low.startswith(b"_atom_site."):
-            raise ValueError(f"CIF file {fn}, line {_line_col(fd, at)[0] + 1}: the _atom_site category is not a loop; "
-                             "only a loop_ of atom rows is read")
+            raise ValueError(f"CIF file {fn}, line {_trajio.line_col(fd, at)[0] + 1}: the _atom_site category is not a "
+                             "loop; only a loop_ of atom rows is read")
     if find_loop and header and header[0].startswith(b"_atom_site."):  # a header that runs to the end of the file: no rows
         return dict(cell=cell, tags=[t[len(b"_atom_site."):].decode("latin-1") for t in header], body=E)
     return dict(cell=cell, tags=None, body=E)
@@ -246,9 +247,9 @@ def _marks(fd: int, body: int, E: int, dev, B: int, T: int, model_col: int):
 
 def _bad_row(fn, fd, pos: int, E: int, T: int, model_col: int) -> ValueError:
     """the error of the row the index pass flagged at file offset ``pos``"""
-    line = _line_at(fd, pos, E)
+    line = _trajio.line_at(fd, pos, E)
     toks, complete = _tokens(line)
-    no = _line_col(fd, pos)[0] + 1
+    no = _trajio.line_col(fd, pos)[0] + 1
     if complete and len(toks) == T:
         if model_col >= 0 and not (not toks[model_col][1] and re.fullmatch(rb"[+-]?[0-9]{1,18}", toks[model_col][0])):
             return ValueError(f"CIF file {fn}, line {no}: the pdbx_PDB_model_num token {toks[model_col][0]!r} is not "
@@ -268,7 +269,7 @@ def index_cif(filename, device=None, chunk_bytes: int = CHUNK_BYTES) -> dict:
     tag), topology (frame 0's rows, with ``pdb.FIELDS`` keys), box and boxangles ((3,) float32: the file's one cell),
     tags (the loop's tags after '_atom_site.', lower case)).  The loop body goes through the device in chunks of
     ``chunk_bytes`` with one host sync at the end.  Errors: see the module docstring."""
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     if chunk_bytes <= 0:
         raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
     B = (int(chunk_bytes) + 15) & ~15
@@ -295,7 +296,7 @@ def index_cif(filename, device=None, chunk_bytes: int = CHUNK_BYTES) -> dict:
             n_rows = term_rank
         errors = []
         if lone_cr < stop:
-            line, col = _line_col(fd, lone_cr)
+            line, col = _trajio.line_col(fd, lone_cr)
             errors.append((lone_cr, ValueError(f"CIF file {fn}, line {line + 1}, column {col}: a CR that is not "
                                                "followed by LF ends a line; lone CR line endings are not supported")))
         if bad < stop:
@@ -315,8 +316,8 @@ def index_cif(filename, device=None, chunk_bytes: int = CHUNK_BYTES) -> dict:
         if len(diff):
             f = int(diff[0])
             raise ValueError(f"CIF file {fn}, frame {f} (model {int(model[f])}, line "
-                             f"{_line_col(fd, int(start[f]))[0] + 1}): {int(count[f])} rows, frame 0 has {N} (every model "
-                             "must hold the same atoms)")
+                             f"{_trajio.line_col(fd, int(start[f]))[0] + 1}): {int(count[f])} rows, frame 0 has {N} "
+                             "(every model must hold the same atoms)")
         end = np.append(start[1:], stop).astype(np.int64)
         raw0 = os.pread(fd, int(end[0] - start[0]), int(start[0]))
         topology = _topology(fn, fd, tags, raw0, int(start[0]))
@@ -369,8 +370,8 @@ def _topology(fn, fd, tags, raw: bytes, base: int) -> dict:
                 x = _value(v, q)
                 out[r] = 0 if x is None else (int(v) if kind is int else x)
             except ValueError:
-                raise ValueError(f"{_where(fn, 0, _line_col(fd, rows[r][0])[0] + 1, i + 1)}: the {tags[i]} token {v!r} "
-                                 f"is not {'an integer' if kind is int else 'a number'}") from None
+                raise ValueError(f"{_where(fn, 0, _trajio.line_col(fd, rows[r][0])[0] + 1, i + 1)}: the {tags[i]} "
+                                 f"token {v!r} is not {'an integer' if kind is int else 'a number'}") from None
         return out
 
     return dict(record=text("group_PDB"), serial=number(int, np.int64, "id"),
@@ -402,16 +403,13 @@ def decode_cif_device(buf: torch.Tensor, n_staged: int, frame_of, natoms: int, c
         out = torch.empty((natoms, 3, F), dtype=torch.float32, device=dev)
     if flags is None:
         flags = torch.zeros(1 + flag_cap, dtype=torch.int64, device=dev)
-    assert out.shape == (natoms, 3, F) and out.dtype == torch.float32 and out.device == dev
-    s_atom, s_axis, s_frame = out.stride()
-    assert F == 0 or (s_atom == 3 * s_axis and (F == 1 or s_frame == 1) and s_axis >= F), \
-        "out must be (natoms, 3, F) frame-minor (a frame slice of a contiguous tensor is fine)"
+    stride = _trajio.decode_outputs(dev, natoms, F, out)
     assert flags.dtype == torch.int64 and flags.device == dev and flags.numel() >= 1 + flag_cap
     if F == 0:
         return out, flags
     cx, cy, cz = (int(c) for c in cols)
     _lib.call(dev, "mkb_cif_decode", _lib.ptr(buf), int(buf.numel()), int(n_staged),
-              frame_of.ctypes.data_as(C.c_void_p), F, int(natoms), cx, cy, cz, _lib.ptr(out), max(int(s_axis), F, 1),
+              frame_of.ctypes.data_as(C.c_void_p), F, int(natoms), cx, cy, cz, _lib.ptr(out), stride,
               int(frame_base), _lib.ptr(flags), int(flag_cap))
     return out, flags
 
@@ -448,13 +446,13 @@ def _host_rows(fn, fd, start, end, sel, N, k, a, cols, tags, coords) -> None:
         if cached[0] != f:
             cached = (f, _rows(os.pread(fd, int(end[f] - start[f]), int(start[f])), int(start[f])))
         pos, ln = cached[1][at]
-        vals[j] = _row_coords(fn, ln, cols, tags, f, lambda: _line_col(fd, pos)[0] + 1)
+        vals[j] = _row_coords(fn, ln, cols, tags, f, lambda: _trajio.line_col(fd, pos)[0] + 1)
     dev = coords.device
     coords[torch.from_numpy(a).to(dev), :, torch.from_numpy(k).to(dev)] = torch.from_numpy(vals).to(dev)
 
 
 def _read(filename, frames, index, device, chunk_bytes):
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     if chunk_bytes <= 0:
         raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
     idx = index if index is not None else index_cif(fn, device, chunk_bytes)
@@ -471,28 +469,16 @@ def _read(filename, frames, index, device, chunk_bytes):
                 model=np.asarray(idx["model"], np.int64)[sel])
     if n == 0:
         return coords, info
-    sizes = end - start
-    chunks = _trajio.chunks(sel, sizes, int(chunk_bytes))
     flags = torch.zeros(1 + FLAG_CAP, dtype=torch.int64, device=dev)
     with open(fn, "rb") as fh:
         fd = fh.fileno()
 
-        def stage(c, host):  # frame j + 1 starts where frame j ends, so a run of frames is one read
-            return int(_trajio.stage_frames(fd, start, sizes, chunks[c][2], host, "CIF")[-1])
+        def decode(buf, at, frame_of, k0, k1):
+            decode_cif_device(buf, len(at) - 1, frame_of, N, cols, out=coords[:, :, k0:k1], flags=flags, frame_base=k0)
 
-        def consume(c, buf):
-            k0, k1, uniq = chunks[c]
-            decode_cif_device(buf, len(uniq), np.searchsorted(uniq, sel[k0:k1]), N, cols, out=coords[:, :, k0:k1],
-                              flags=flags, frame_base=k0)
-
-        _trajio.upload(dev, len(chunks), max(int(sizes[u].sum()) for _, _, u in chunks), stage, consume)
-        n_host = int(flags[0].item())
-        if n_host:
-            if n_host <= FLAG_CAP:
-                ent = flags[1:1 + n_host].cpu().numpy()
-                k, a = ent // N, ent % N
-            else:  # too many to list: every row of the listed frames
-                k, a = np.divmod(np.arange(n * N, dtype=np.int64), N)
+        _trajio.read_frames(fd, dev, sel, start, end - start, chunk_bytes, "CIF", decode)
+        k, a, _ = _trajio.flagged(flags, n, N, FLAG_CAP, 1)
+        if len(k):
             _host_rows(fn, fd, start, end, sel, N, k, a, cols, idx["tags"], coords)
             info["host_lines"] = len(k)
     return coords, info
@@ -649,9 +635,9 @@ def _prepare(coords, topology, box, boxangles, title, device, chunk_bytes):
     box, angles = cell
     if box is not None and angles is None:
         angles = np.full((3, F), 90.0, np.float32)
-    t = _fields(topology, natoms)
+    t = topology_fields(topology, natoms)
     layout = _layout(t, natoms, F)
-    bad = _first_bad(coords, *COORD, 1000)
+    bad = _trajio.first_bad(coords, *COORD, 1000)
     if bad is not None:
         f, atom, axis, v = bad
         raise ValueError(f"coords at frame {f}, atom {atom}, axis {'xyz'[axis]} is {v!r}: a '%10.3f' Cartn field "
@@ -730,7 +716,7 @@ def write_cif(filename, coords, topology, box=None, boxangles=None, title=None, 
     printable ASCII that can be quoted; resid and charge integers; occupancy and beta finite; a row of at most 768
     bytes.  The frames are encoded in chunks of at most ``chunk_bytes`` and each chunk is written while the next one
     encodes.  The file is created or truncated."""
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     x, natoms, F, head, layout = _prepare(coords, topology, box, boxangles, title, device, chunk_bytes)
     with open(fn, "wb") as fh:
         _emit(fh, x, natoms, F, head, layout, chunk_bytes)

@@ -290,10 +290,7 @@ def decode_dcd_device(buf: torch.Tensor, frames: np.ndarray, natoms: int, swap: 
     F = int(frames.shape[0])
     if out is None:
         out = torch.empty((natoms, 3, F), dtype=torch.float32, device=dev)
-    assert out.shape == (natoms, 3, F) and out.dtype == torch.float32 and out.device == dev
-    s_atom, s_axis, s_frame = out.stride()
-    assert natoms == 0 or F == 0 or (s_atom == 3 * s_axis and (F == 1 or s_frame == 1) and s_axis >= F), \
-        "out must be (natoms, 3, F) frame-minor (a frame slice of a contiguous tensor is fine)"
+    stride = _trajio.decode_outputs(dev, natoms, F, out)
     if F == 0 or natoms == 0:
         return out
     first_arr = None
@@ -304,7 +301,7 @@ def decode_dcd_device(buf: torch.Tensor, frames: np.ndarray, natoms: int, swap: 
     _lib.call(dev, "mkb_dcd_decode", _lib.ptr(buf), int(buf.numel()), frames.ctypes.data_as(C.c_void_p), F, int(natoms),
               _lib.ptr(slot), int(n_free), _lib.ptr(first_buf), int(first_buf.numel()) if first_buf is not None else 0,
               first_arr.ctypes.data_as(C.c_void_p) if first_arr is not None else None, int(bool(swap)), _lib.ptr(out),
-              int(s_axis) if F > 1 else max(int(s_axis), 1))
+              stride)
     return out
 
 
@@ -330,7 +327,6 @@ def read_dcd_device(filename, frames=None, device=None, chunk_bytes: int = CHUNK
     if n == 0 or natoms == 0:
         return coords, idx["box"][:, sel], idx["boxangles"][:, sel], info
     start, size, fdesc = idx["start"], idx["size"], idx["frames"]
-    chunks = _trajio.chunks(sel, size, int(chunk_bytes))
     with open(filename, "rb") as fh:
         slot = first_buf = first = None
         if idx["free"] is not None:  # the first frame stays resident: it holds the fixed atoms of every frame
@@ -339,21 +335,14 @@ def read_dcd_device(filename, frames=None, device=None, chunk_bytes: int = CHUNK
             first = fdesc[:1].copy()
             first["offset"] -= start[0]
             slot = torch.from_numpy(_slot_map(natoms, idx["free"])).to(dev)
-        staged = {}
 
-        def stage(c, host):
-            staged[c] = _trajio.stage_frames(fh.fileno(), start, size, chunks[c][2], host, "DCD")
-            return int(staged[c][-1])
-
-        def consume(c, buf):
-            k0, k1, uniq = chunks[c]
-            at = staged.pop(c)
+        def decode(buf, at, frame_of, k0, k1):
             desc = fdesc[sel[k0:k1]].copy()
-            desc["offset"] += (at[np.searchsorted(uniq, sel[k0:k1])] - start[sel[k0:k1]])[:, None]
+            desc["offset"] += (at[frame_of] - start[sel[k0:k1]])[:, None]
             decode_dcd_device(buf, desc, natoms, idx["swap"], slot, natoms - idx["namnf"], first_buf, first,
                               out=coords[:, :, k0:k1])
 
-        _trajio.upload(dev, len(chunks), max(int(size[u].sum()) for _, _, u in chunks), stage, consume)
+        _trajio.read_frames(fh.fileno(), dev, sel, start, size, chunk_bytes, "DCD", decode)
     return coords, idx["box"][:, sel], idx["boxangles"][:, sel], info
 
 

@@ -63,7 +63,6 @@ import numpy as np
 import torch
 
 from . import _lib, _trajio
-from .xyz import _content_end, _line_at, _line_col
 
 logger = logging.getLogger(__name__)
 
@@ -79,10 +78,6 @@ BOX = (-9999999, 99999999)  # rint(b * 10^5): '%10.5f' with a leading space, so 
 ORDER = ((0, 0), (1, 1), (2, 2), (0, 1), (0, 2), (1, 0), (1, 2), (2, 0), (2, 1))  # GRO's box fields as (vector, axis)
 FIELD_NAMES = ("x", "y", "z", "vx", "vy", "vz")
 WS = b" \t\n\v\f\r"  # the whitespace bytes.split(), int() and float() take (not 0x1c-0x1f, unlike str.split())
-
-
-def _name(filename) -> str:
-    return filename.decode("UTF-8") if isinstance(filename, bytes) else str(filename)
 
 
 def _where(fn, frame: int, line: int, col: int) -> str:
@@ -237,14 +232,14 @@ def _index(fn, fd, E: int, head: dict, dev, B: int) -> dict:
     flagged = np.flatnonzero(status[1:F].cpu().numpy()) + 1
     errors = []
     if lone_cr != INT64_MAX:
-        line, col = _line_col(fd, lone_cr)
+        line, col = _trajio.line_col(fd, lone_cr)
         errors.append((lone_cr, ValueError(f"{_where(fn, line // P, line + 1, col)}: a CR that is not followed by LF "
                                            "ends a line; lone CR line endings are not supported")))
     for f in flagged.tolist():
-        title = _line_at(fd, int(offsets[f]), E)
+        title = _trajio.line_at(fd, int(offsets[f]), E)
         pos = int(offsets[f]) + len(title) + 1
         try:
-            _count(fn, _strip_cr(_line_at(fd, pos, E)), f, f * P + 2, natoms)
+            _count(fn, _strip_cr(_trajio.line_at(fd, pos, E)), f, f * P + 2, natoms)
         except ValueError as e:
             errors.append((pos, e))
             break
@@ -261,11 +256,11 @@ def index_gro(filename, device=None, chunk_bytes: int = CHUNK_BYTES) -> dict:
     (frame 0's resid, resname, name and serial)).  The file goes through the device in chunks of ``chunk_bytes`` with
     one host sync at the end.  Count-line mismatches, inconsistent decimal spacing and lone CR line endings raise
     ValueError (see the module docstring)."""
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     if chunk_bytes <= 0:
         raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
     with open(fn, "rb") as fh:
-        E = _content_end(fh.fileno(), os.fstat(fh.fileno()).st_size)
+        E = _trajio.content_end(fh.fileno(), os.fstat(fh.fileno()).st_size)
         if E == 0:
             raise ValueError(f"GRO file {fn}: no frames (the file is empty or blank)")
         return _index(fn, fh.fileno(), E, _frame0(fn, fh, E), _lib.device(device), (int(chunk_bytes) + 15) & ~15)
@@ -293,20 +288,13 @@ def decode_gro_device(buf: torch.Tensor, n_staged: int, frame_of, natoms: int, w
         raise ValueError("velocities requested from a file without velocities")
     if flags is None:
         flags = torch.zeros(1 + flag_cap, dtype=torch.int64, device=dev)
-    for t in (out, vout):
-        if t is None:
-            continue
-        assert t.shape == (natoms, 3, F) and t.dtype == torch.float32 and t.device == dev
-        s_atom, s_axis, s_frame = t.stride()
-        assert F == 0 or (s_atom == 3 * s_axis and (F == 1 or s_frame == 1) and s_axis >= F), \
-            "out must be (natoms, 3, F) frame-minor (a frame slice of a contiguous tensor is fine)"
-    assert vout is None or F == 0 or vout.stride(1) == out.stride(1), "out and vout must share their strides"
+    stride = _trajio.decode_outputs(dev, natoms, F, out, vout)
     assert flags.dtype == torch.int64 and flags.device == dev and flags.numel() >= 1 + flag_cap
     if F == 0:
         return out, vout, flags
     _lib.call(dev, "mkb_gro_decode", _lib.ptr(buf), int(buf.numel()), int(n_staged),
               frame_of.ctypes.data_as(C.c_void_p), F, int(natoms), int(width), int(bool(velocities)), _lib.ptr(out),
-              _lib.ptr(vout), max(int(out.stride(1)), F, 1), int(frame_base), _lib.ptr(flags), int(flag_cap))
+              _lib.ptr(vout), stride, int(frame_base), _lib.ptr(flags), int(flag_cap))
     return out, vout, flags
 
 
@@ -332,7 +320,7 @@ def _check_fields(fields) -> tuple:
 
 
 def _read(filename, frames, fields, scale, index, device, chunk_bytes):
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     fields = _check_fields(fields)
     if chunk_bytes <= 0:
         raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
@@ -342,7 +330,7 @@ def _read(filename, frames, fields, scale, index, device, chunk_bytes):
     with open(fn, "rb") as fh:
         fd = fh.fileno()
         if index is None:
-            E = _content_end(fd, os.fstat(fd).st_size)
+            E = _trajio.content_end(fd, os.fstat(fd).st_size)
             if E == 0:
                 raise ValueError(f"GRO file {fn}: no frames (the file is empty or blank)")
             head = _frame0(fn, fh, E)
@@ -367,21 +355,15 @@ def _read(filename, frames, fields, scale, index, device, chunk_bytes):
         out = {k: t for k, t in (("x", x), ("v", v)) if k in fields}
         if n == 0:
             return out, box, info
-        sizes = np.diff(offs)
-        chunks = _trajio.chunks(sel, sizes, int(chunk_bytes))
         flags = torch.zeros(1 + FLAG_CAP, dtype=torch.int64, device=dev)
         heads = []
 
-        def stage(c, host):
-            return int(_trajio.stage_frames(fd, offs[:-1], sizes, chunks[c][2], host, "GRO")[-1])
-
-        def consume(c, buf):
-            k0, k1, uniq = chunks[c]
-            decode_gro_device(buf, len(uniq), np.searchsorted(uniq, sel[k0:k1]), N, w, vel, out=x[:, :, k0:k1],
+        def decode(buf, at, frame_of, k0, k1):
+            decode_gro_device(buf, len(at) - 1, frame_of, N, w, vel, out=x[:, :, k0:k1],
                               vout=None if v is None else v[:, :, k0:k1], flags=flags, frame_base=k0)
-            heads.append(_head_device(buf, np.concatenate([[0], np.cumsum(sizes[uniq])]), dev))
+            heads.append(_head_device(buf, at, dev))
 
-        _trajio.upload(dev, len(chunks), max(int(sizes[u].sum()) for _, _, u in chunks), stage, consume)
+        chunks = _trajio.read_frames(fd, dev, sel, offs[:-1], np.diff(offs), chunk_bytes, "GRO", decode)
         box9 = np.empty((n, 9), np.float32)
         errors = []  # (1-based line, ValueError): the first bad box line and the first bad atom line
         for (k0, k1, uniq), (b_d, t_d, s_d, st_d) in zip(chunks, heads):
@@ -405,13 +387,8 @@ def _read(filename, frames, fields, scale, index, device, chunk_bytes):
                     info["step"][k0 + j] = _step(_strip_cr(raw[0]))
         for t, (i, j) in enumerate(ORDER):
             box[i, j] = box9[:, t]
-        n_host = int(flags[0].item())
-        if n_host:
-            if n_host <= FLAG_CAP:
-                ent = flags[1:1 + n_host].cpu().numpy()
-                k, a = ent // N, ent % N
-            else:  # too many to list: every atom line of the listed frames
-                k, a = np.divmod(np.arange(n * N, dtype=np.int64), N)
+        k, a, _ = _trajio.flagged(flags, n, N, FLAG_CAP, 1)
+        if len(k):
             bad = _host_lines(fn, fd, offs, sel, N, w, 6 if vel else 3, k, a, x, v)
             if bad is not None:
                 errors.append(bad)
@@ -525,26 +502,6 @@ def _prefix(t: dict, natoms: int) -> np.ndarray:
     return np.frombuffer(b.tobytes(), np.uint8).copy()
 
 
-def _first_bad(a, lo: int, hi: int, scale: float):
-    """the first (frame, atom, axis, value) of (natoms, 3, F) ``a`` in file order with rint(x * scale) outside [lo, hi]
-    or not finite, else None; one min / max pass when every value is inside"""
-    if a.numel() == 0 if isinstance(a, torch.Tensor) else a.size == 0:
-        return None
-    if isinstance(a, torch.Tensor):
-        mn, mx = (float(v) for v in torch.stack(torch.aminmax(a)).cpu())
-    else:
-        with np.errstate(invalid="ignore"):
-            mn, mx = a.min(), a.max()
-    if np.rint(np.float64(mn) * scale) >= lo and np.rint(np.float64(mx) * scale) <= hi:
-        return None
-    x = a.cpu().numpy() if isinstance(a, torch.Tensor) else a
-    with np.errstate(invalid="ignore", over="ignore"):
-        k = np.rint(x.astype(np.float64) * scale)
-        bad = ~((k >= lo) & (k <= hi))
-    f, atom, axis = np.unravel_index(np.argmax(bad.transpose(2, 0, 1)), (x.shape[2], x.shape[0], 3))
-    return int(f), int(atom), int(axis), float(x[atom, axis, f])
-
-
 def _per_frame(v, F: int, name: str, dtype):
     """``v`` (None, a scalar or one value per frame) -> (F,) float64, or int64 for ``dtype`` int; integer input is
     taken as int64 as it is, so steps past 2^53 keep every digit"""
@@ -603,10 +560,10 @@ def _prepare(coords, topology, box, time, step, title, velocities, device, chunk
     steps = _per_frame(step, F, "step", int)
     t = _fields(topology, natoms)
     prefix = _prefix(t, natoms)
-    bad = [(b, what) for b, what in ((_first_bad(coords, *COORD, 1000), "coords"),
-                                     (_first_bad(velocities, *VELOCITY, 10000) if velocities is not None else None,
-                                      "velocities"),
-                                     (_first_bad(box, *BOX, 100000), "box")) if b is not None]
+    bad = [(b, what) for b, what in ((_trajio.first_bad(coords, *COORD, 1000), "coords"),
+                                     (_trajio.first_bad(velocities, *VELOCITY, 10000) if velocities is not None
+                                      else None, "velocities"),
+                                     (_trajio.first_bad(box, *BOX, 100000), "box")) if b is not None]
     if bad:
         (f, atom, axis, v), what = min(bad, key=lambda e: (e[0][0], e[1] != "coords", e[1] == "box"))
         field = dict(coords="'%8.3f' (-999.999 to 9999.999)", velocities="'%8.4f' (-99.9999 to 999.9999)",
@@ -716,7 +673,7 @@ def write_gro(filename, coords, topology, box, time=None, step=None, title: str 
     name at most 5 ASCII characters without whitespace; resid >= 0; the title ASCII without a line break; integer
     steps within int64.  The frames are encoded in chunks of at most ``chunk_bytes`` and each chunk is written while
     the next one encodes.  The file is created or truncated."""
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     prep = _prepare(coords, topology, box, time, step, title, velocities, device, chunk_bytes)
     with open(fn, "wb") as fh:
         _emit(fh, *prep, chunk_bytes)

@@ -49,17 +49,12 @@ logger = logging.getLogger(__name__)
 CHUNK_BYTES = 256 << 20
 MAX_ATOMS = (2**31 - 1) // 3
 INT64_MAX = 2**63 - 1
-WS = b" \t\n\v\f\r\x1c\x1d\x1e\x1f"  # the ASCII bytes str.split() splits on
 G9_MAX = 15  # longest '%.9g' of a float32
 STYLES = ("x", "xu", "xs", "xsu")
 TRIPLES = {"x": ("x", "y", "z"), "xu": ("xu", "yu", "zu"), "xs": ("xs", "ys", "zs"), "xsu": ("xsu", "ysu", "zsu")}
 BLOCKS = {"v": ("vx", "vy", "vz"), "f": ("fx", "fy", "fz")}
 ROLE_ID, ROLE_POS, ROLE_IMG, ROLE_VEL, ROLE_FRC = 1, 2, 5, 8, 11
 _FIELD = re.compile(r"\S+")
-
-
-def _name(filename) -> str:
-    return filename.decode("UTF-8") if isinstance(filename, bytes) else str(filename)
 
 
 def _where(fn, frame: int, line: int, col: int) -> str:
@@ -71,30 +66,6 @@ def _text(fn, raw: bytes, frame: int, line: int) -> str:
         return raw.decode("utf-8").rstrip("\r")
     except UnicodeDecodeError as e:
         raise ValueError(f"{_where(fn, frame, line, e.start + 1)}: the line is not UTF-8 text") from None
-
-
-def _content_end(fd: int, size: int) -> int:
-    """one past the last byte that is not ASCII whitespace (0 for a blank file)"""
-    end, step = size, 1 << 16
-    while end > 0:
-        lo = max(0, end - step)
-        tail = os.pread(fd, end - lo, lo).rstrip(WS)
-        if tail:
-            return lo + len(tail)
-        end = lo
-    return 0
-
-
-def _line_col(fd: int, pos: int) -> tuple[int, int]:
-    """0-based line and 1-based column of file offset ``pos``"""
-    lines, last, step = 0, -1, 64 << 20
-    for w in range(0, pos, step):
-        b = np.frombuffer(os.pread(fd, min(step, pos - w), w), np.uint8)
-        nl = np.flatnonzero(b == 10)
-        lines += len(nl)
-        if len(nl):
-            last = w + int(nl[-1])
-    return lines, pos - last
 
 
 class _Lines:
@@ -362,7 +333,7 @@ def _index(fn, fd: int, E: int, h0: dict, dev, B: int) -> dict:
     steps[0], times[0], bnd[0] = h0["step"], h0["time"], h0["bounds"]
     errors = []
     if lone_cr != INT64_MAX:
-        line, col = _line_col(fd, lone_cr)
+        line, col = _trajio.line_col(fd, lone_cr)
         errors.append((lone_cr, ValueError(f"{_where(fn, max(0, (line - u) // P), line + 1, col)}: a CR that is not "
                                            "followed by LF ends a line; lone CR line endings are not supported")))
     flagged = np.flatnonzero(status[1:F].cpu().numpy() | hstatus[1:F].cpu().numpy()) + 1
@@ -391,12 +362,12 @@ def index_lammpstrj(filename, device=None, chunk_bytes: int = CHUNK_BYTES) -> di
     the file offset of each frame and the end of the last), columns, units, step (F,) int64, time (F,) float64 (NaN
     without ITEM: TIME), bounds (F, 3, 3) float64 (the raw bound lines), ids, type (and mol, element when present:
     frame 0's, in ascending id order)).  Errors: see the module docstring."""
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     if chunk_bytes <= 0:
         raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
     with open(fn, "rb") as fh:
         fd = fh.fileno()
-        E = _content_end(fd, os.fstat(fd).st_size)
+        E = _trajio.content_end(fd, os.fstat(fd).st_size)
         if E == 0:
             raise ValueError(f"LAMMPS dump file {fn}: no frames (the file is empty or blank)")
         h0 = _frame0(fn, fd, E)
@@ -493,15 +464,9 @@ def decode_lammpstrj_device(buf: torch.Tensor, n_staged: int, frame_of, natoms: 
     role = torch.as_tensor(np.asarray(role, np.int8)).to(dev)
     if fstat is None:
         fstat = torch.zeros(max(4, (F + 3) & ~3), dtype=torch.uint8, device=dev)
-    strides = {int(t.stride(1)) for t in (out, vout, fout) if t is not None}
-    for t in (out, vout, fout):
-        assert t is None or (t.shape == (natoms, 3, F) and t.dtype == torch.float32 and t.device == dev)
-        assert t is None or F <= 1 or (t.stride(2) == 1 and t.stride(0) == 3 * t.stride(1)), \
-            "out must be (natoms, 3, F) frame-minor (a frame slice of a contiguous tensor is fine)"
-    assert len(strides) <= 1, "out, vout and fout must share one frame stride"
+    stride = _trajio.decode_outputs(dev, natoms, F, out, vout, fout)
     if F == 0:
         return out, vout, fout, fstat
-    stride = max(strides.pop() if strides else F, F)
     _lib.call(dev, "mkb_lammpstrj_decode", _lib.ptr(buf), int(buf.numel()), int(n_staged),
               frame_of.ctypes.data_as(C.c_void_p), F, int(natoms), int(H), _lib.ptr(role), int(role.numel()),
               _lib.ptr(ids) if ids is not None else None, _lib.ptr(params) if params is not None else None,
@@ -512,7 +477,7 @@ def decode_lammpstrj_device(buf: torch.Tensor, n_staged: int, frame_of, natoms: 
 
 
 def _read(filename, frames, fields, style, unwrap, scale, index, device, chunk_bytes):
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     if chunk_bytes <= 0:
         raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
     s = np.float32(scale)
@@ -522,7 +487,7 @@ def _read(filename, frames, fields, style, unwrap, scale, index, device, chunk_b
         fd = fh.fileno()
         dev = _lib.device(device)
         if index is None:
-            E = _content_end(fd, os.fstat(fd).st_size)
+            E = _trajio.content_end(fd, os.fstat(fd).st_size)
             if E == 0:
                 raise ValueError(f"LAMMPS dump file {fn}: no frames (the file is empty or blank)")
             h0 = _frame0(fn, fd, E)
@@ -552,21 +517,15 @@ def _read(filename, frames, fields, style, unwrap, scale, index, device, chunk_b
         dense = "id" not in cols or np.array_equal(idx["ids"], np.arange(1, N + 1))
         ids_d = None if dense else torch.from_numpy(np.ascontiguousarray(idx["ids"], np.int64)).to(dev)
         params_d = torch.from_numpy(params).to(dev)
-        sizes = np.diff(offs)
-        chunks = _trajio.chunks(sel, sizes, int(chunk_bytes))
         stats = []
 
-        def stage(c, host):
-            return int(_trajio.stage_frames(fd, offs[:-1], sizes, chunks[c][2], host, "LAMMPS dump")[-1])
-
-        def consume(c, buf):
-            k0, k1, uniq = chunks[c]
+        def decode(buf, at, frame_of, k0, k1):
             _, _, _, st = decode_lammpstrj_device(
-                buf, len(uniq), np.searchsorted(uniq, sel[k0:k1]), N, H, role, ids_d, params_d[k0:k1],
-                style in ("xs", "xsu"), add, *(out[k][:, :, k0:k1] if k in out else None for k in ("x", "v", "f")))
+                buf, len(at) - 1, frame_of, N, H, role, ids_d, params_d[k0:k1], style in ("xs", "xsu"), add,
+                *(out[k][:, :, k0:k1] if k in out else None for k in ("x", "v", "f")))
             stats.append(st)
 
-        _trajio.upload(dev, len(chunks), max(int(sizes[u].sum()) for _, _, u in chunks), stage, consume)
+        chunks = _trajio.read_frames(fd, dev, sel, offs[:-1], np.diff(offs), chunk_bytes, "LAMMPS dump", decode)
         fst = np.concatenate([st.cpu().numpy()[:k1 - k0] for st, (k0, k1, _) in zip(stats, chunks)])
         redo = np.flatnonzero(fst)
         if len(redo):
@@ -801,7 +760,7 @@ def write_lammpstrj(filename, coords, box, step=None, time=None, ids=None, types
     float(np.float32(v)) (NaN and infinities as Python spells them).  The frames are encoded in chunks of at most
     ``chunk_bytes`` and each chunk is written while the next one encodes.  The file is created or truncated; every
     argument is checked before it is opened."""
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     args = _prepare(coords, box, step, time, ids, types, velocities, origin, units, device, chunk_bytes)
     with open(fn, "wb") as fh:
         _emit(fh, *args, chunk_bytes)

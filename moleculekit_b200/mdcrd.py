@@ -129,10 +129,7 @@ def decode_mdcrd_device(buf: torch.Tensor, offsets, natoms: int, with_box: bool,
         box_out = torch.empty((3, F), dtype=torch.float32, device=dev)
     if bad is None:
         bad = torch.full((1,), INT64_MAX, dtype=torch.int64, device=dev)
-    assert out.shape == (natoms, 3, F) and out.dtype == torch.float32 and out.device == dev
-    s_atom, s_axis, s_frame = out.stride()
-    assert F == 0 or (s_atom == 3 * s_axis and (F == 1 or s_frame == 1) and s_axis >= F), \
-        "out must be (natoms, 3, F) frame-minor (a frame slice of a contiguous tensor is fine)"
+    stride = _trajio.decode_outputs(dev, natoms, F, out)
     box_stride = 1
     if with_box:
         assert box_out.shape == (3, F) and box_out.dtype == torch.float32 and box_out.device == dev
@@ -142,7 +139,7 @@ def decode_mdcrd_device(buf: torch.Tensor, offsets, natoms: int, with_box: bool,
     if F == 0:
         return out, box_out, bad
     _lib.call(dev, "mkb_mdcrd_decode", _lib.ptr(buf), int(buf.numel()), offsets.ctypes.data_as(C.c_void_p), F,
-              int(natoms), int(bool(with_box)), _lib.ptr(out), max(int(s_axis), F, 1),
+              int(natoms), int(bool(with_box)), _lib.ptr(out), stride,
               _lib.ptr(box_out if with_box else None), box_stride, _lib.ptr(bad))
     return out, box_out, bad
 
@@ -267,35 +264,15 @@ def _writer_args(coords, box, title, chunk_bytes):
     return natoms, F
 
 
-def _writable(lo, hi) -> bool:
-    """the extremes of an array (NaN when it holds one) -> every value is writable"""
-    return bool(np.rint(np.float64(lo) * 1000) >= NEG_MIN and np.rint(np.float64(hi) * 1000) <= POS_MAX)
-
-
 def _check_range(a, name: str) -> None:
     """ValueError naming the first value of ``a`` ((natoms, 3, F) coords or (3, F) box) in file order that '%8.3f'
-    cannot write in 8 characters; one min / max pass when every value is writable"""
-    if a.numel() == 0 if isinstance(a, torch.Tensor) else a.size == 0:
-        return
-    if isinstance(a, torch.Tensor):
-        lo, hi = (float(v) for v in torch.stack(torch.aminmax(a)).cpu())
-    else:
-        with np.errstate(invalid="ignore"):
-            lo, hi = a.min(), a.max()
-    if _writable(lo, hi):
-        return
-    x = a.cpu().numpy() if isinstance(a, torch.Tensor) else a
-    with np.errstate(invalid="ignore", over="ignore"):
-        k = np.rint(x.astype(np.float64) * 1000)
-        bad = ~((k >= NEG_MIN) & (k <= POS_MAX))
-    if x.ndim == 3:
-        f, atom, axis = np.unravel_index(np.argmax(bad.transpose(2, 0, 1)), (x.shape[2], x.shape[0], 3))
-        where, v = f"frame {f}, atom {atom}, axis {'xyz'[axis]}", x[atom, axis, f]
-    else:
-        f, axis = np.unravel_index(np.argmax(bad.T), (x.shape[1], 3))
-        where, v = f"frame {f}, axis {'ABC'[axis]}", x[axis, f]
-    raise ValueError(f"{name} at {where} is {float(v)!r}: an mdcrd field (%8.3f) holds -999.999 to 9999.999 and no "
-                     "NaN or infinity")
+    cannot write in 8 characters"""
+    bad = _trajio.first_bad(a, NEG_MIN, POS_MAX, 1000)
+    if bad is not None:
+        f, atom, axis, v = bad
+        where = f"frame {f}, atom {atom}, axis {'xyz'[axis]}" if atom is not None else f"frame {f}, axis {'ABC'[axis]}"
+        raise ValueError(f"{name} at {where} is {v!r}: an mdcrd field (%8.3f) holds -999.999 to 9999.999 and no NaN "
+                         "or infinity")
 
 
 def _prepare(coords, box, title, device, chunk_bytes):

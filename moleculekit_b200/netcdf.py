@@ -268,14 +268,11 @@ def decode_netcdf_device(buf: torch.Tensor, offsets, natoms: int, out: torch.Ten
     F = int(offsets.shape[0])
     if out is None:
         out = torch.empty((natoms, 3, F), dtype=torch.float32, device=dev)
-    assert out.shape == (natoms, 3, F) and out.dtype == torch.float32 and out.device == dev
-    s_atom, s_axis, s_frame = out.stride()
-    assert natoms == 0 or F == 0 or (s_atom == 3 * s_axis and (F == 1 or s_frame == 1) and s_axis >= F), \
-        "out must be (natoms, 3, F) frame-minor (a frame slice of a contiguous tensor is fine)"
+    stride = _trajio.decode_outputs(dev, natoms, F, out)
     if F == 0 or natoms == 0:
         return out
     _lib.call(dev, "mkb_netcdf_decode", _lib.ptr(buf), int(buf.numel()), offsets.ctypes.data_as(C.c_void_p), F,
-              int(natoms), _lib.ptr(out), int(s_axis) if F > 1 else max(int(s_axis), 1))
+              int(natoms), _lib.ptr(out), stride)
     return out
 
 

@@ -54,7 +54,6 @@ import numpy as np
 import torch
 
 from . import _lib, _trajio
-from .xyz import _line_at, _line_col
 
 logger = logging.getLogger(__name__)
 
@@ -74,10 +73,6 @@ COORD = (-999999, 9999999)  # rint(x * 1000) that '%8.3f' writes in 8 characters
 LENGTH = (-9999999, 99999999)  # rint(x * 1000), '%9.3f'
 ANGLE = (-99999, 999999)  # rint(x * 100), '%7.2f'
 OCCUPANCY = (-9999, 99999)  # rint(x * 100), '%6.2f'
-
-
-def _name(filename) -> str:
-    return filename.decode("UTF-8") if isinstance(filename, bytes) else str(filename)
 
 
 def _where(fn, frame: int, line: int, col: int) -> str:
@@ -133,7 +128,7 @@ def index_pdb(filename, device=None, chunk_bytes: int = CHUNK_BYTES) -> dict:
     each frame's CRYST1 record, -1 without one), topology (frame 0's atom records, see the module docstring)).  The file
     goes through the device in chunks of ``chunk_bytes`` with one host sync at the end.  Frames whose atom count is not
     frame 0's and lone CR line endings raise ValueError (see the module docstring)."""
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     if chunk_bytes <= 0:
         raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
     B = (int(chunk_bytes) + 15) & ~15
@@ -157,13 +152,14 @@ def index_pdb(filename, device=None, chunk_bytes: int = CHUNK_BYTES) -> dict:
         count = (a1 - a0).astype(np.int64)
         errors = []
         if lone_cr != INT64_MAX:
-            line, col = _line_col(fd, lone_cr)
+            line, col = _trajio.line_col(fd, lone_cr)
             errors.append((lone_cr, ValueError(f"PDB file {fn}, line {line + 1}, column {col}: a CR that is not "
                                                "followed by LF ends a line; lone CR line endings are not supported")))
         N = int(count[0])
         if N == 0:
-            errors.append((int(start[0]), ValueError(f"PDB file {fn}: frame 0 (line {_line_col(fd, int(start[0]))[0] + 1}"
-                                                     ") holds no ATOM or HETATM record")))
+            line = _trajio.line_col(fd, int(start[0]))[0] + 1
+            errors.append((int(start[0]), ValueError(f"PDB file {fn}: frame 0 (line {line}) holds no ATOM or HETATM "
+                                                     "record")))
         F = len(count)
         if F > 1 and not closed[-1] and count[-1] < N:
             F -= 1
@@ -172,8 +168,8 @@ def index_pdb(filename, device=None, chunk_bytes: int = CHUNK_BYTES) -> dict:
         bad = np.flatnonzero(count[:F] != N)
         if len(bad) and N:
             f = int(bad[0])
-            line, _ = _line_col(fd, int(start[f]))
-            serial = _line_at(fd, int(start[f]), E)[6:].strip().decode("latin-1")
+            line, _ = _trajio.line_col(fd, int(start[f]))
+            serial = _trajio.line_at(fd, int(start[f]), E)[6:].strip().decode("latin-1")
             errors.append((int(start[f]), ValueError(
                 f"PDB file {fn}, frame {f} (MODEL {serial}, line {line + 1}): {int(count[f])} atom records, frame 0 "
                 f"has {N} (every model must hold the same atoms)")))
@@ -195,7 +191,7 @@ def _int_field(fn, fd, pos, line: bytes, a: int, b: int, what: str) -> int:
     try:
         return int(s)
     except ValueError:
-        raise ValueError(f"{_where(fn, 0, _line_col(fd, pos)[0] + 1, a + 1)}: the {what} {s!r} is not an "
+        raise ValueError(f"{_where(fn, 0, _trajio.line_col(fd, pos)[0] + 1, a + 1)}: the {what} {s!r} is not an "
                          "integer") from None
 
 
@@ -206,7 +202,7 @@ def _float_field(fn, fd, pos, line: bytes, a: int, b: int, what: str) -> float:
     try:
         return float(s)
     except ValueError:
-        raise ValueError(f"{_where(fn, 0, _line_col(fd, pos)[0] + 1, a + 1)}: the {what} {s!r} is not a "
+        raise ValueError(f"{_where(fn, 0, _trajio.line_col(fd, pos)[0] + 1, a + 1)}: the {what} {s!r} is not a "
                          "number") from None
 
 
@@ -217,8 +213,8 @@ def _charge(fn, fd, pos, line: bytes) -> float:
     try:
         return float(int(s[:-1]) * (-1 if s[-1:] == b"-" else 1)) if s[-1:] in (b"+", b"-") else float(int(s))
     except ValueError:
-        raise ValueError(f"{_where(fn, 0, _line_col(fd, pos)[0] + 1, 79)}: the charge {s!r} is not an integer with "
-                         "an optional trailing sign") from None
+        raise ValueError(f"{_where(fn, 0, _trajio.line_col(fd, pos)[0] + 1, 79)}: the charge {s!r} is not an integer "
+                         "with an optional trailing sign") from None
 
 
 def _topology(fn, raw: bytes, base: int, fd: int) -> dict:
@@ -258,16 +254,13 @@ def decode_pdb_device(buf: torch.Tensor, n_staged: int, frame_of, natoms: int, o
         out = torch.empty((natoms, 3, F), dtype=torch.float32, device=dev)
     if flags is None:
         flags = torch.zeros(1 + flag_cap, dtype=torch.int64, device=dev)
-    assert out.shape == (natoms, 3, F) and out.dtype == torch.float32 and out.device == dev
-    s_atom, s_axis, s_frame = out.stride()
-    assert F == 0 or (s_atom == 3 * s_axis and (F == 1 or s_frame == 1) and s_axis >= F), \
-        "out must be (natoms, 3, F) frame-minor (a frame slice of a contiguous tensor is fine)"
+    stride = _trajio.decode_outputs(dev, natoms, F, out)
     assert flags.dtype == torch.int64 and flags.device == dev and flags.numel() >= 1 + flag_cap
     if F == 0:
         return out, flags
     _lib.call(dev, "mkb_pdb_decode", _lib.ptr(buf), int(buf.numel()), int(n_staged),
-              frame_of.ctypes.data_as(C.c_void_p), F, int(natoms), _lib.ptr(out), max(int(s_axis), F, 1),
-              int(frame_base), _lib.ptr(flags), int(flag_cap))
+              frame_of.ctypes.data_as(C.c_void_p), F, int(natoms), _lib.ptr(out), stride, int(frame_base),
+              _lib.ptr(flags), int(flag_cap))
     return out, flags
 
 
@@ -305,7 +298,7 @@ def _host_lines(fn, fd, start, end, sel, N, k, a, coords) -> None:
                 pos += len(ln) + 1
             cached = (f, rows)
         pos, ln = cached[1][at]
-        vals[j] = _atom_coords(fn, ln, f, lambda: _line_col(fd, pos)[0] + 1)
+        vals[j] = _atom_coords(fn, ln, f, lambda: _trajio.line_col(fd, pos)[0] + 1)
     dev = coords.device
     coords[torch.from_numpy(a).to(dev), :, torch.from_numpy(k).to(dev)] = torch.from_numpy(vals).to(dev)
 
@@ -330,9 +323,9 @@ def _cells(fn, fd, E: int, cell: np.ndarray, dev):
     _lib.call(dev, "mkb_pdb_cell", _lib.ptr(rows_d), len(pos), _lib.ptr(cells_d), _lib.ptr(bad_d))
     cells = cells_d.cpu().numpy().reshape(-1, 6)
     for i in np.flatnonzero(bad_d.cpu().numpy()).tolist():  # the host decides, and names a bad field
-        line = _line_at(fd, int(pos[i]), E)
+        line = _trajio.line_at(fd, int(pos[i]), E)
         line = line[:-1] if line.endswith(b"\r") else line
-        line_no = _line_col(fd, int(pos[i]))[0] + 1
+        line_no = _trajio.line_col(fd, int(pos[i]))[0] + 1
         if len(line) < 54:
             raise ValueError(f"PDB file {fn}, line {line_no}, column {len(line) + 1}: the CRYST1 record has "
                              f"{len(line)} columns, it needs 54: {line!r}")
@@ -349,23 +342,8 @@ def _cells(fn, fd, E: int, cell: np.ndarray, dev):
     return np.ascontiguousarray(picked[:, :3].T), np.ascontiguousarray(picked[:, 3:].T)
 
 
-def _stage(fd, start, end, uniq, host) -> int:
-    """the frames ``uniq`` back to back into ``host`` (one read per run of frames that touch in the file)"""
-    at = 0
-    k = 0
-    while k < len(uniq):
-        j = k
-        while j + 1 < len(uniq) and uniq[j + 1] == uniq[j] + 1 and start[uniq[j + 1]] == end[uniq[j]]:
-            j += 1
-        n = int(end[uniq[j]] - start[uniq[k]])
-        _trajio.read_exact(fd, host[at:at + n], int(start[uniq[k]]), "PDB")
-        at += n
-        k = j + 1
-    return at
-
-
 def _read(filename, frames, index, device, chunk_bytes):
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     if chunk_bytes <= 0:
         raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
     idx = index if index is not None else index_pdb(fn, device, chunk_bytes)
@@ -379,30 +357,18 @@ def _read(filename, frames, index, device, chunk_bytes):
                 box=np.zeros((3, n), np.float32), boxangles=np.full((3, n), 90.0, np.float32))
     if n == 0:
         return coords, info
-    sizes = end - start
-    chunks = _trajio.chunks(sel, sizes, int(chunk_bytes))
     flags = torch.zeros(1 + FLAG_CAP, dtype=torch.int64, device=dev)
     with open(fn, "rb") as fh:
         fd = fh.fileno()
 
-        def stage(c, host):
-            return _stage(fd, start, end, chunks[c][2], host)
+        def decode(buf, at, frame_of, k0, k1):
+            decode_pdb_device(buf, len(at) - 1, frame_of, N, out=coords[:, :, k0:k1], flags=flags, frame_base=k0)
 
-        def consume(c, buf):
-            k0, k1, uniq = chunks[c]
-            decode_pdb_device(buf, len(uniq), np.searchsorted(uniq, sel[k0:k1]), N, out=coords[:, :, k0:k1],
-                              flags=flags, frame_base=k0)
-
-        _trajio.upload(dev, len(chunks), max(int(sizes[u].sum()) for _, _, u in chunks), stage, consume)
+        _trajio.read_frames(fd, dev, sel, start, end - start, chunk_bytes, "PDB", decode)
         E = os.fstat(fd).st_size
         info["box"], info["boxangles"] = _cells(fn, fd, E, np.asarray(idx["cell"], np.int64)[sel], dev)
-        n_host = int(flags[0].item())
-        if n_host:
-            if n_host <= FLAG_CAP:
-                ent = flags[1:1 + n_host].cpu().numpy()
-                k, a = ent // N, ent % N
-            else:  # too many to list: every atom line of the listed frames
-                k, a = np.divmod(np.arange(n * N, dtype=np.int64), N)
+        k, a, _ = _trajio.flagged(flags, n, N, FLAG_CAP, 1)
+        if len(k):
             _host_lines(fn, fd, start, end, sel, N, k, a, coords)
             info["host_lines"] = len(k)
     return coords, info
@@ -430,7 +396,7 @@ def read_pdb_frames(filename, frames, index: dict | None = None, device=None, ch
 
 
 # ------------------------------------------------------------------------------------------------------------ writing
-def _fields(topology, natoms: int) -> dict:
+def topology_fields(topology, natoms: int) -> dict:
     """``topology`` (a Molecule / MolLite-like object or a dict) -> a dict of the FIELDS as natoms-long arrays; a
     missing field takes the reader's blank default (serial: 1 ... natoms)"""
     def get(k):
@@ -449,6 +415,9 @@ def _fields(topology, natoms: int) -> dict:
             raise ValueError(f"topology field {k} has {len(v)} entries, coords have {natoms} atoms")
         out[k] = v
     return out
+
+
+_fields = topology_fields  # the name bench_pdb.py, bench_cif.py and the tests build writer templates with
 
 
 def _check_topology(t: dict, natoms: int) -> None:
@@ -520,29 +489,6 @@ def _template(t: dict, natoms: int) -> np.ndarray:
     return out
 
 
-def _first_bad(a, lo: int, hi: int, scale: float):
-    """the first (frame, atom-or-None, axis) of (natoms, 3, F) or (3, F) ``a`` in file order with rint(x * scale)
-    outside [lo, hi] or not finite, else None; one min / max pass when every value is inside"""
-    if a.numel() == 0 if isinstance(a, torch.Tensor) else a.size == 0:
-        return None
-    if isinstance(a, torch.Tensor):
-        mn, mx = (float(v) for v in torch.stack(torch.aminmax(a)).cpu())
-    else:
-        with np.errstate(invalid="ignore"):
-            mn, mx = a.min(), a.max()
-    if np.rint(np.float64(mn) * scale) >= lo and np.rint(np.float64(mx) * scale) <= hi:
-        return None
-    x = a.cpu().numpy() if isinstance(a, torch.Tensor) else a
-    with np.errstate(invalid="ignore", over="ignore"):
-        k = np.rint(x.astype(np.float64) * scale)
-        bad = ~((k >= lo) & (k <= hi))
-    if x.ndim == 3:
-        f, atom, axis = np.unravel_index(np.argmax(bad.transpose(2, 0, 1)), (x.shape[2], x.shape[0], 3))
-        return int(f), int(atom), int(axis), float(x[atom, axis, f])
-    f, axis = np.unravel_index(np.argmax(bad.T), (x.shape[1], 3))
-    return int(f), None, int(axis), float(x[axis, f])
-
-
 def _prepare(coords, topology, box, boxangles, device, chunk_bytes):
     """every check, then (coords, box, angles as CUDA tensors or None without frames, natoms, F, template)"""
     coords = _trajio.writer_coords(coords, "write_pdb")
@@ -573,12 +519,12 @@ def _prepare(coords, topology, box, boxangles, device, chunk_bytes):
     box, angles = cell
     if box is not None and angles is None:
         angles = np.full((3, F), 90.0, np.float32)
-    t = _fields(topology, natoms)
+    t = topology_fields(topology, natoms)
     _check_topology(t, natoms)
-    bad = [(b, what) for b, what in ((_first_bad(coords, *COORD, 1000), "coords"),) if b is not None]
+    bad = [(b, what) for b, what in ((_trajio.first_bad(coords, *COORD, 1000), "coords"),) if b is not None]
     if box is not None:
-        bad += [(b, what) for b, what in ((_first_bad(box, *LENGTH, 1000), "box"),
-                                          (_first_bad(angles, *ANGLE, 100), "boxangles")) if b is not None]
+        bad += [(b, what) for b, what in ((_trajio.first_bad(box, *LENGTH, 1000), "box"),
+                                          (_trajio.first_bad(angles, *ANGLE, 100), "boxangles")) if b is not None]
     if bad:
         (f, atom, axis, v), what = min(bad, key=lambda e: (e[0][0], e[1] == "coords"))
         field = dict(coords="'%8.3f' (-999.999 to 9999.999)", box="'%9.3f' (-9999.999 to 99999.999)",
@@ -664,7 +610,7 @@ def write_pdb(filename, coords, topology, box=None, boxangles=None, device=None,
     segid at most 4 characters, chain, altloc and insertion 1, element 2, record ATOM or HETATM; resid within '%4d';
     occupancy and beta within '%6.2f'; charge an integer from -9 to 9.  The frames are encoded in chunks of at most
     ``chunk_bytes`` and each chunk is written while the next one encodes.  The file is created or truncated."""
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     x, b, ang, natoms, F, tmpl = _prepare(coords, topology, box, boxangles, device, chunk_bytes)
     with open(fn, "wb") as fh:
         _emit(fh, x, b, ang, natoms, F, tmpl, chunk_bytes)

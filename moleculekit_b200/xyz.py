@@ -47,52 +47,7 @@ MAX_ELEMENT = 256  # widest element column the writer takes
 FLAG_CAP = 1 << 20  # host lines recorded by position per read; past it every atom line of the listed frames is re-read
 INT64_MAX = 2**63 - 1
 POS_MAX, NEG_MIN = 99999999999999, -9999999999999  # rint(x * 1e8) that '%15.8f' writes in 15 characters
-WS = b" \t\n\v\f\r\x1c\x1d\x1e\x1f"  # the ASCII bytes str.split() splits on
 _FIELD = re.compile(r"\S+")
-
-
-def _name(filename) -> str:
-    return filename.decode("UTF-8") if isinstance(filename, bytes) else str(filename)
-
-
-def _content_end(fd: int, size: int) -> int:
-    """one past the last byte that is not ASCII whitespace (0 for a blank file)"""
-    end, step = size, 1 << 16
-    while end > 0:
-        lo = max(0, end - step)
-        tail = os.pread(fd, end - lo, lo).rstrip(WS)
-        if tail:
-            return lo + len(tail)
-        end = lo
-    return 0
-
-
-def _line_at(fd: int, pos: int, end: int) -> bytes:
-    """the bytes of the line starting at file offset ``pos``, without its '\\n' (not past ``end``)"""
-    out, step = b"", 4096
-    while pos < end:
-        b = os.pread(fd, min(step, end - pos), pos)
-        if not b:
-            break
-        i = b.find(b"\n")
-        if i >= 0:
-            return out + b[:i]
-        out += b
-        pos += len(b)
-        step *= 2
-    return out
-
-
-def _line_col(fd: int, pos: int) -> tuple[int, int]:
-    """0-based line and 1-based column of file offset ``pos`` (counts the newlines before it)"""
-    lines, last, step = 0, -1, 64 << 20
-    for w in range(0, pos, step):
-        b = np.frombuffer(os.pread(fd, min(step, pos - w), w), np.uint8)
-        nl = np.flatnonzero(b == 10)
-        lines += len(nl)
-        if len(nl):
-            last = w + int(nl[-1])
-    return lines, pos - last
 
 
 def _where(fn, frame: int, line: int, col: int) -> str:
@@ -161,13 +116,13 @@ def index_xyz(filename, device=None, chunk_bytes: int = CHUNK_BYTES) -> dict:
     file offset of each frame and the end of the last), element (list of str: field 0 of frame 0's atom lines), comment
     (str: frame 0's comment line)).  The file goes through the device in chunks of ``chunk_bytes`` with one host sync at
     the end.  Count-line mismatches and lone CR line endings raise ValueError (see the module docstring)."""
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     if chunk_bytes <= 0:
         raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
     B = (int(chunk_bytes) + 15) & ~15
     with open(fn, "rb") as fh:
         fd = fh.fileno()
-        E = _content_end(fd, os.fstat(fd).st_size)
+        E = _trajio.content_end(fd, os.fstat(fd).st_size)
         if E == 0:
             raise ValueError(f"XYZ file {fn}: no frames (the file is empty or blank)")
         natoms, comment, element = _frame0(fn, fh, E)
@@ -200,12 +155,12 @@ def index_xyz(filename, device=None, chunk_bytes: int = CHUNK_BYTES) -> dict:
         flagged = np.flatnonzero(status[1:F].cpu().numpy()) + 1
         errors = []
         if lone_cr != INT64_MAX:
-            line, col = _line_col(fd, lone_cr)
+            line, col = _trajio.line_col(fd, lone_cr)
             errors.append((lone_cr, ValueError(f"{_where(fn, line // P, line + 1, col)}: a CR that is not followed by "
                                                "LF ends a line; lone CR line endings are not supported")))
         for f in flagged.tolist():
             try:
-                _count(fn, _line_at(fd, int(offsets[f]), E), f, f * P + 1, natoms)
+                _count(fn, _trajio.line_at(fd, int(offsets[f]), E), f, f * P + 1, natoms)
             except ValueError as e:
                 errors.append((int(offsets[f]), e))
                 break
@@ -246,21 +201,18 @@ def decode_xyz_device(buf: torch.Tensor, n_staged: int, frame_of, natoms: int, o
         out = torch.empty((natoms, 3, F), dtype=torch.float32, device=dev)
     if flags is None:
         flags = torch.zeros(1 + 2 * flag_cap, dtype=torch.int64, device=dev)
-    assert out.shape == (natoms, 3, F) and out.dtype == torch.float32 and out.device == dev
-    s_atom, s_axis, s_frame = out.stride()
-    assert F == 0 or (s_atom == 3 * s_axis and (F == 1 or s_frame == 1) and s_axis >= F), \
-        "out must be (natoms, 3, F) frame-minor (a frame slice of a contiguous tensor is fine)"
+    stride = _trajio.decode_outputs(dev, natoms, F, out)
     assert flags.dtype == torch.int64 and flags.device == dev and flags.numel() >= 1 + 2 * flag_cap
     if F == 0:
         return out, flags
     _lib.call(dev, "mkb_xyz_decode", _lib.ptr(buf), int(buf.numel()), int(n_staged),
-              frame_of.ctypes.data_as(C.c_void_p), F, int(natoms), _lib.ptr(out), max(int(s_axis), F, 1),
-              int(frame_base), _lib.ptr(flags), int(flag_cap))
+              frame_of.ctypes.data_as(C.c_void_p), F, int(natoms), _lib.ptr(out), stride, int(frame_base),
+              _lib.ptr(flags), int(flag_cap))
     return out, flags
 
 
 def _read(filename, frames, index, device, chunk_bytes):
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     if chunk_bytes <= 0:
         raise ValueError(f"chunk_bytes must be positive, got {chunk_bytes}")
     idx = index if index is not None else index_xyz(fn, device, chunk_bytes)
@@ -272,29 +224,16 @@ def _read(filename, frames, index, device, chunk_bytes):
     info = dict(natoms=N, n_frames=F, frames=sel, element=list(idx["element"]), comment=idx["comment"], host_lines=0)
     if n == 0:
         return coords, info
-    sizes = np.diff(offs)
-    chunks = _trajio.chunks(sel, sizes, int(chunk_bytes))
     flags = torch.zeros(1 + 2 * FLAG_CAP, dtype=torch.int64, device=dev)
     with open(fn, "rb") as fh:
         fd = fh.fileno()
 
-        def stage(c, host):
-            return int(_trajio.stage_frames(fd, offs[:-1], sizes, chunks[c][2], host, "XYZ")[-1])
+        def decode(buf, at, frame_of, k0, k1):
+            decode_xyz_device(buf, len(at) - 1, frame_of, N, out=coords[:, :, k0:k1], flags=flags, frame_base=k0)
 
-        def consume(c, buf):
-            k0, k1, uniq = chunks[c]
-            decode_xyz_device(buf, len(uniq), np.searchsorted(uniq, sel[k0:k1]), N, out=coords[:, :, k0:k1],
-                              flags=flags, frame_base=k0)
-
-        _trajio.upload(dev, len(chunks), max(int(sizes[u].sum()) for _, _, u in chunks), stage, consume)
-        n_host = int(flags[0].item())
-        if n_host:
-            if n_host <= FLAG_CAP:
-                ent = flags[1:1 + 2 * n_host].view(n_host, 2).cpu().numpy()
-                k, a, rel = ent[:, 0] // N, ent[:, 0] % N, ent[:, 1]
-            else:  # too many to list: every atom line of the listed frames
-                k, a = np.divmod(np.arange(n * N, dtype=np.int64), N)
-                rel = None
+        _trajio.read_frames(fd, dev, sel, offs[:-1], np.diff(offs), chunk_bytes, "XYZ", decode)
+        k, a, rel = _trajio.flagged(flags, n, N, FLAG_CAP, 2)
+        if len(k):
             _host_lines(fn, fd, offs, sel, N, k, a, rel, coords)
             info["host_lines"] = len(k)
     return coords, info
@@ -313,7 +252,7 @@ def _host_lines(fn, fd, offs, sel, N, k, a, rel, coords) -> None:
                 frame_lines = {f: os.pread(fd, int(offs[f + 1] - offs[f]), int(offs[f])).split(b"\n")}
             raw = frame_lines[f][2 + at]
         else:
-            raw = _line_at(fd, int(offs[f] + rel[j]), int(offs[f + 1]))
+            raw = _trajio.line_at(fd, int(offs[f] + rel[j]), int(offs[f + 1]))
         vals[j] = _atom(fn, raw, f, f * (N + 2) + 3 + at)
     dev = coords.device
     coords[torch.from_numpy(a).to(dev), :, torch.from_numpy(k).to(dev)] = torch.from_numpy(vals).to(dev)
@@ -367,23 +306,12 @@ def _writer_args(coords, element, comment, chunk_bytes):
 
 def _check_range(a) -> None:
     """ValueError naming the first value of (natoms, 3, F) ``a`` in file order that '%15.8f' cannot write in 15
-    characters; one min / max pass when every value is writable"""
-    if a.numel() == 0 if isinstance(a, torch.Tensor) else a.size == 0:
-        return
-    if isinstance(a, torch.Tensor):
-        lo, hi = (float(v) for v in torch.stack(torch.aminmax(a)).cpu())
-    else:
-        with np.errstate(invalid="ignore"):
-            lo, hi = a.min(), a.max()
-    if np.rint(np.float64(lo) * 1e8) >= NEG_MIN and np.rint(np.float64(hi) * 1e8) <= POS_MAX:
-        return
-    x = a.cpu().numpy() if isinstance(a, torch.Tensor) else a
-    with np.errstate(invalid="ignore", over="ignore"):
-        k = np.rint(x.astype(np.float64) * 1e8)
-        bad = ~((k >= NEG_MIN) & (k <= POS_MAX))
-    f, atom, axis = np.unravel_index(np.argmax(bad.transpose(2, 0, 1)), (x.shape[2], x.shape[0], 3))
-    raise ValueError(f"coords at frame {f}, atom {atom}, axis {'xyz'[axis]} is {float(x[atom, axis, f])!r}: an XYZ "
-                     "field (%15.8f) holds -99999.99999999 to 999999.99999999 and no NaN or infinity")
+    characters"""
+    bad = _trajio.first_bad(a, NEG_MIN, POS_MAX, 1e8)
+    if bad is not None:
+        f, atom, axis, v = bad
+        raise ValueError(f"coords at frame {f}, atom {atom}, axis {'xyz'[axis]} is {v!r}: an XYZ field (%15.8f) holds "
+                         "-99999.99999999 to 999999.99999999 and no NaN or infinity")
 
 
 def _prepare(coords, element, comment, device, chunk_bytes):
@@ -455,7 +383,7 @@ def write_xyz(filename, coords, element, comment: str = "", device=None, chunk_b
     -99999.99999999), NaN or +-inf is rejected with an error naming the first offending frame, atom and axis.  The
     frames are encoded in chunks of at most ``chunk_bytes`` and each chunk is written while the next one encodes.  The
     file is created or truncated; arguments and values are checked before it is opened."""
-    fn = _name(filename)
+    fn = _trajio.name(filename)
     x, natoms, F, head, column = _prepare(coords, element, comment, device, chunk_bytes)
     with open(fn, "wb") as fh:
         _emit(fh, x, natoms, F, head, column, chunk_bytes)
